@@ -1,7 +1,7 @@
 #!/usr/bin/env python
-"""bench.py -- BASELINE.json's metric on BASELINE.json's config, on B200.
+"""bench.py -- BASELINE.json's metric on BASELINE.json's config, on H100.
 
-    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--skip-configs]
+    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--skip-configs] [--dump-outputs DIR]
 
 metric  : XSimGCL yelp2018 train steps/sec (+ full-catalog rank items/sec as `rank`)
 workload: configs[2] of BASELINE.json -- XSimGCL, yelp2018 shape (31 668 x 38 048 x 1 237 259, synthetic power-law
@@ -17,10 +17,16 @@ e2e     = the same metric through the public API with HOST buffers, every step: 
           Same measurement at every N.
 Other configs of BASELINE.json ride along as sub-records of the same JSON line: `config2` (LightGCN yelp2018),
 `config4` (SGL edge-drop, amazon-kindle shape, view graphs rebuilt on the device), `config5` (SimGCL, synthetic
-10 M x 2 M x 200 M, d = 128; single GPU at N = 1, bipartite-sharded at N > 1).
---impl reference times the reference's own CPU path on the host cores: the UNMODIFIED reference unpacked from
-baseline/_ref/reference.zip (kind "reference") when that archive travelled, else the op-for-op port
-oracle/torch_port.py (kind "port"); rank 0 only; best of a thread-count sweep.
+5 M x 1 M x 100 M, d = 128 -- the largest synthetic shape of the recipe that one 80 GB GPU holds; single GPU at N = 1,
+bipartite-sharded at N > 1).
+--impl reference times K steps (after W warm-up steps) of the reference's CPU path on the host cores through its
+op-for-op port oracle/torch_port.py (kind "port"); rank 0 only; thread count = best of a short sweep.
+--dump-outputs DIR (N = 1): after the timed steps, writes what the last timed step computed -- the trained tables
+user_emb.npy / item_emb.npy and the step's losses.npy, float32 -- so that two builds can be compared output for
+output.  Data, batches, initial tables and Philox noise are seeded: the same arguments give the same inputs.  The
+summation order of the float atomics (gradient scatter, InfoNCE split reductions) is not fixed, and over hundreds of
+Adam steps that shows in the tables (~10 % relative between two runs of one build at --steps 200, where the losses
+agree to ~2e-5): compare tables with a short --steps, losses at any length.
 """
 import argparse
 import json
@@ -38,7 +44,6 @@ sys.path.insert(0, ROOT)
 CFG = dict(model="XSimGCL", shape="yelp2018", d=64, L=3, B=2048, tau=0.2, lam=0.2, eps=0.2, l_star=1, lr=1e-3, reg=1e-4)
 METRIC = "XSimGCL yelp2018 train steps/sec"
 WORKLOAD = "XSimGCL yelp2018-shape 31668x38048x1237259, L=3 d=64 B=2048 tau=0.2 lambda=0.2 eps=0.2 l*=1"
-TRAFFIC_FILE = os.path.join("profiles", "r02_spmm_traffic.json")  # dram bytes per launch from this round's ncu capture
 
 _JSON_OUT = None
 
@@ -65,17 +70,18 @@ def log(msg):
 
 
 def peaks():
-    """Roofline denominators: the driver-measured copy bandwidth and cuBLAS bf16 rate of this pool's B200s."""
+    """Roofline denominators: MEASURED_PEAKS.json (measured copy bandwidth and bf16 rate of the machine) when present,
+    else NVIDIA's H100 SXM data-sheet figures (700 W part) -- a bound, not a measurement."""
     p = os.path.join(ROOT, "MEASURED_PEAKS.json")
     if os.path.exists(p):
         with open(p) as f:
             d = json.load(f)
-        return {"hbm_gbs": float(d["hbm_gbs"]), "bf16_tflops": float(d.get("bf16_tflops", 1702.0)), "source": "measured (MEASURED_PEAKS.json)"}
-    return {"hbm_gbs": 6650.0, "bf16_tflops": 1700.0, "source": "fallback (B200_PROFILING.md)"}
+        return {"hbm_gbs": float(d["hbm_gbs"]), "bf16_tflops": float(d.get("bf16_tflops", 989.0)), "source": "measured (MEASURED_PEAKS.json)"}
+    return {"hbm_gbs": 3350.0, "bf16_tflops": 989.0, "source": "fallback (H100 SXM data sheet, dense)"}
 
 
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons DURING the timed region (B200_PROFILING.md recipe)."""
+    """nvidia-smi clocks / throttle reasons DURING the timed region."""
 
     Q = ("index,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.active,clocks_event_reasons.hw_slowdown,"
          "clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap")
@@ -191,50 +197,28 @@ THREADS = (8, 16, 32, 64, 128)
 
 
 class CpuPath:
-    """The reference's CPU path for the bench workload: the unmodified reference when its archive travelled, else the
-    port.  run(steps, warmup) -> seconds; rank() -> (seconds, users, items)."""
+    """The reference's CPU path for the bench workload, through its op-for-op port (oracle/torch_port.py).
+    run(steps, warmup) -> seconds; rank() -> (seconds, users, items)."""
 
     def __init__(self, data):
+        import random
         import torch
         sys.path.insert(0, os.path.join(ROOT, "oracle"))
-        import refarchive
+        import torch_port
         self.torch = torch
         self.kind = "port"
-        self.scratch = tempfile.mkdtemp(prefix="srb_ref_")
-        if refarchive.available():
-            try:
-                import ref_runner
-                cwd = os.getcwd()
-                root = refarchive.unpack(os.path.join(self.scratch, "reference"))
-                self.ref = ref_runner.ReferenceXSimGCL(root, os.path.join(self.scratch, "run"), data.pair_users, data.pair_items, d=CFG["d"],
-                                                       L=CFG["L"], B=CFG["B"], lr=CFG["lr"], reg=CFG["reg"], eps=CFG["eps"], tau=CFG["tau"],
-                                                       lam=CFG["lam"], l_star=CFG["l_star"], test_users=1000)
-                os.chdir(cwd)
-                self.kind = "reference"
-            except Exception as e:  # noqa: BLE001 -- the port is the documented fallback of the reference arm
-                log(f"unmodified reference unusable ({type(e).__name__}: {e}); using the port")
-        if self.kind == "port":
-            import random
-            import torch_port
-            random.seed(0)
-            self.tp = torch_port
-            self.m = torch_port.XSimGCLCpu(data.norm_adj.tocsr(), data.user_num, data.item_num, CFG["d"], CFG["L"], CFG["eps"], CFG["tau"],
-                                           CFG["lam"], CFG["l_star"], CFG["lr"], CFG["reg"])
-            rp, ri = data.rated_csr()
-            self.rp, self.ri = rp, ri
-            self.rated = [set(ri[rp[u]:rp[u + 1]].tolist()) for u in range(data.user_num)]
-            perm = np.random.default_rng(0).permutation(len(data.pair_users))
-            self.pu, self.pi, self.ptr = data.pair_users[perm], data.pair_items[perm], 0
-            self.data = data
+        random.seed(0)
+        self.tp = torch_port
+        self.m = torch_port.XSimGCLCpu(data.norm_adj.tocsr(), data.user_num, data.item_num, CFG["d"], CFG["L"], CFG["eps"], CFG["tau"],
+                                       CFG["lam"], CFG["l_star"], CFG["lr"], CFG["reg"])
+        rp, ri = data.rated_csr()
+        self.rp, self.ri = rp, ri
+        self.rated = [set(ri[rp[u]:rp[u + 1]].tolist()) for u in range(data.user_num)]
+        perm = np.random.default_rng(0).permutation(len(data.pair_users))
+        self.pu, self.pi, self.ptr = data.pair_users[perm], data.pair_items[perm], 0
+        self.data = data
 
     def run(self, steps, warmup):
-        if self.kind == "reference":
-            cwd = os.getcwd()
-            os.chdir(os.path.join(self.scratch, "run"))
-            try:
-                return self.ref.time_steps(steps, max(warmup, 1))
-            finally:
-                os.chdir(cwd)
         def one():
             u, i, j, self.ptr = self.tp.sample_batch(self.pu, self.pi, self.ptr, CFG["B"], self.data.item_num, self.rated)
             if self.ptr >= len(self.pu):
@@ -248,13 +232,6 @@ class CpuPath:
         return time.perf_counter() - t0
 
     def rank(self):
-        if self.kind == "reference":
-            cwd = os.getcwd()
-            os.chdir(os.path.join(self.scratch, "run"))
-            try:
-                return self.ref.time_rank()
-            finally:
-                os.chdir(cwd)
         import oracle
         ue, ie = self.m.ue.detach().numpy(), self.m.ie.detach().numpy()
         sample = np.arange(0, self.data.user_num, max(1, self.data.user_num // 1000))[:1000]
@@ -283,16 +260,11 @@ def run_reference(args, rank, world):
     data = build_data()
     cpu = CpuPath(data)
     best, table = cpu.sweep()
-    steps = min(args.steps, 20)
-    warm = min(max(args.warmup, 1), 5)
-    # bounded: keep the whole arm within a few minutes whatever the host
-    per_step = 1.0 / table[best]
-    steps = max(2, min(steps, int(60.0 / per_step)))
+    steps, warm = args.steps, args.warmup  # the host path is slow (about 2 s per step): choose --steps accordingly
     dt = cpu.run(steps, warm)
     val = steps / dt
     rdt, r_users, r_items = cpu.rank()
-    note = ("UNMODIFIED reference (baseline/_ref/reference.zip): its own XSimGCL.train() loop, sampler, losses, torch.optim.Adam"
-            if cpu.kind == "reference" else "op-for-op port of the reference's CPU path (oracle/torch_port.py) incl. Python sampler")
+    note = "op-for-op port of the reference's CPU path (oracle/torch_port.py) incl. Python sampler"
     line = {
         "impl": "reference", "metric": METRIC, "value": val, "unit": "steps/s", "n_gpus": args.gpus, "steps": steps, "warmup": warm,
         "ms_per_step": 1e3 * dt / steps, "higher_is_better": True, "scaling": "weak" if args.gpus == 1 else "strong", "vs_baseline": None,
@@ -316,8 +288,8 @@ def cpu_baseline(data, budget_s=45.0):
     dt = cpu.run(steps, 1)
     return {"value": steps / dt, "unit": "steps/s", "cores": best, "kind": cpu.kind, "host_cores": os.cpu_count(),
             "thread_sweep_steps_per_s": {str(k): v for k, v in table.items()},
-            "sample": f"{steps} full XSimGCL train steps ({'unmodified reference, its own train() loop' if cpu.kind == 'reference' else 'oracle/torch_port.py'}"
-                      f", torch CPU, Python sampler) after 1 warm-up; thread count = best of the sweep"}
+            "sample": f"{steps} full XSimGCL train steps (oracle/torch_port.py, torch CPU, Python sampler) after 1 warm-up; "
+                      "thread count = best of the sweep"}
 
 
 # ------------------------------------------------------------------------------------------
@@ -404,14 +376,15 @@ def record_config4(args, dev):
 
 
 def record_config5(args, dev, world, rank, dist):
-    """configs[4]: SimGCL on the synthetic 10 M x 2 M x 200 M bipartite graph (SURVEY 8d recipe: Zipf(1.1) on both
+    """configs[4]: SimGCL on the synthetic 5 M x 1 M x 100 M bipartite graph (SURVEY 8d recipe: Zipf(1.1) on both
     sides, de-duplicated, first-appearance ids; generated, assembled and normalised on the GPU), d=128, L=3, B=2048,
     eps=0.1, lambda=0.5, tau=0.2.  N = 1: the single-GPU engine; N > 1: bipartite-sharded.  SRB_CONFIG5=<shape>
-    selects another shape (e.g. synthetic-2M, the mid-size stand-in)."""
+    selects another shape (synthetic-10M, BASELINE.json's original size, needs more than one 80 GB GPU;
+    synthetic-2M is the mid-size stand-in)."""
     import torch
     from selfrec_b200 import ops, synth
     from selfrec_b200.shard_check import device_batches, sharded_vs_single
-    shape_name = os.environ.get("SRB_CONFIG5", "synthetic-10M")
+    shape_name = os.environ.get("SRB_CONFIG5", "synthetic-5M")
     U, I, nnz = synth.SHAPES[shape_name]
     d, L, B = 128, 3, 2048
     kw = dict(eps=0.1, tau=0.2, cl_rate=0.5)
@@ -423,7 +396,7 @@ def record_config5(args, dev, world, rank, dist):
     adj = data.norm_adj
     N, nnzA = adj.shape[0], adj.nnz
     rec.update(n=N, nnzA=nnzA, split_rows=adj.n_huge, split_row_chunks=adj.n_work)
-    steps = max(3, min(args.steps, 10))
+    steps = args.steps
     pool = device_batches(data, B, 8, seed=5, dev=dev)
     pk = peaks()
     alg = spmm_bytes(N, nnzA, d)
@@ -444,18 +417,9 @@ def record_config5(args, dev, world, rank, dist):
         sp_ms = e0.elapsed_time(e1) / 4
         del x, y
         torch.cuda.empty_cache()
-        traffic = None
-        tp = os.path.join(ROOT, TRAFFIC_FILE)
-        if os.path.exists(tp):
-            with open(tp) as f:
-                traffic = json.load(f).get(shape_name)
         rec["spmm"] = {"kernel": "spmm_hub_kernel<128> + spmm_csr_kernel<128>", "ms_per_launch": sp_ms, "algorithmic_bytes": alg,
                        "achieved_gbs": alg / sp_ms / 1e6, "frac_of_hbm": alg / sp_ms / 1e6 / pk["hbm_gbs"],
-                       "gather_bytes": 4 * nnzA * d, "gather_gbs": 4 * nnzA * d / sp_ms / 1e6, "dram_traffic": traffic,
-                       "traffic_source": TRAFFIC_FILE if traffic else None,
-                       # what the memory system actually moves: on a graph without community structure every non-zero whose
-                       # column is not among the ~200 k rows L2 can hold costs a 512-byte DRAM read (DESIGN 4.1)
-                       "dram_frac_of_hbm": (traffic / sp_ms / 1e6 / pk["hbm_gbs"]) if traffic else None}
+                       "gather_bytes": 4 * nnzA * d, "gather_gbs": 4 * nnzA * d / sp_ms / 1e6}
         torch.manual_seed(5)
         eng = TrainEngine("SimGCL", data, d, L, B, 1e-3, 1e-4, device=dev, philox_seed=55, **kw)
         g = eng.capture()
@@ -508,6 +472,17 @@ def record_config5(args, dev, world, rank, dist):
 # ------------------------------------------------------------------------------------------
 # our arm, N = 1
 # ------------------------------------------------------------------------------------------
+def dump_outputs(out_dir, eng):
+    """What the last timed step hands its caller: the updated embedding tables and the step's losses, float32
+    (yelp2018 shape: 17.8 MB in all)."""
+    import torch
+    torch.cuda.synchronize()
+    os.makedirs(out_dir, exist_ok=True)
+    for name, t in (("user_emb", eng.user_emb), ("item_emb", eng.item_emb), ("losses", eng.losses)):
+        np.save(os.path.join(out_dir, f"{name}.npy"), t.detach().to("cpu", torch.float32).numpy())
+    log(f"outputs of the last timed step written to {out_dir}")
+
+
 def run_single(args, local_rank):
     import random
     import torch
@@ -562,6 +537,8 @@ def run_single(args, local_rank):
         resident_step(k)
     clocks.start()
     ms = time_steps(resident_step, args.steps, 0, torch)
+    if args.dump_outputs:
+        dump_outputs(args.dump_outputs, eng)
     keep_load(resident_step, ms / args.steps, torch)  # nvidia-smi needs ~0.4 s of this same load to see it
     clk = clocks.stop()
     clk["window"] = "timed region + 0.4 s of the same graph-replay loop (keep_load)"
@@ -570,7 +547,7 @@ def run_single(args, local_rank):
     # same loop with an L2 flush between iterations, per-step events (extra evidence)
     flush = torch.empty(256 * 1024 * 1024 // 4, device=dev, dtype=torch.float32)
     per = []
-    for k in range(min(args.steps, 20)):
+    for k in range(args.steps):
         flush.fill_(float(k))
         e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
         e0.record()
@@ -615,11 +592,6 @@ def run_single(args, local_rank):
     spmm_ms = e0.elapsed_time(e1) / (2 * R)
     alg = spmm_bytes(N, nnzA, CFG["d"])
     achieved = alg / (spmm_ms * 1e-3) / 1e9
-    traffic = None
-    tp = os.path.join(ROOT, TRAFFIC_FILE)
-    if os.path.exists(tp):
-        with open(tp) as f:
-            traffic = json.load(f).get("yelp2018")
     sbytes = step_bytes("XSimGCL", N, nnzA, CFG["d"], CFG["L"])
 
     # ---- rank metric, on TRAINED tables (two epochs through the public API) ----
@@ -634,7 +606,7 @@ def run_single(args, local_rank):
     rpd, rid = torch.from_numpy(rp).to(dev), torch.from_numpy(ri).to(dev)
     rank = {}
     fb_users = None
-    for impl, tag in ((2, "tcgen05 tf32 candidates + exact fp32 rescoring"), (1, "cuda-core fp32")):
+    for impl, tag in ((2, "wgmma tf32 candidates + exact fp32 rescoring"), (1, "cuda-core fp32")):
         ops.score_topk(ue, ie, users, rpd, rid, 20, impl=impl)
         torch.cuda.synchronize()
         e0.record()
@@ -659,7 +631,7 @@ def run_single(args, local_rank):
         "ms_per_step": ms / args.steps, "higher_is_better": True, "scaling": "strong", "vs_baseline": None, "dtype": "f32",
         "data": "synthetic",
         "config": {"workload": WORKLOAD, "parallelism": "single GPU (the N > 1 runs shard this same job: strong scaling)",
-                   "l2": "no flush: per-step working set ~180 MB > 126 MB L2 (see value_l2_flushed)",
+                   "l2": "no flush: per-step working set ~180 MB > 50 MB L2 (see value_l2_flushed)",
                    "inputs": f"{P} pre-sampled batches resident in HBM, CUDA-graph replay"},
         "clocks": clk,
         "e2e": {"value": e2e_val, "unit": "steps/s", "h2d_bytes_per_step": int(eng.words * 4), "d2h_bytes_per_step": 16,
@@ -667,13 +639,11 @@ def run_single(args, local_rank):
         "gpu_launches": int(launches_per_step * args.steps), "launches_per_step": int(launches_per_step),
         "value_l2_flushed": 1e3 / ms_flushed, "ms_per_step_l2_flushed": ms_flushed,
         "roofline": {"bound": "hbm", "kernel": "spmm_csr_kernel<64>", "achieved": achieved, "peak": pk["hbm_gbs"], "unit": "GB/s",
-                     "frac": achieved / pk["hbm_gbs"], "traffic": traffic, "traffic_source": TRAFFIC_FILE if traffic else None,
-                     "peak_source": pk["source"], "ms_per_launch": spmm_ms, "algorithmic_bytes_per_launch": alg,
-                     # what actually bounds this kernel at yelp2018 size: X is L2-resident and every non-zero gathers one
-                     # 256-byte row out of L2 (ceiling measured by tools/l2_microbench.cu, profiles/r01a_l2_gather_microbench.txt)
+                     "frac": achieved / pk["hbm_gbs"], "peak_source": pk["source"], "ms_per_launch": spmm_ms,
+                     "algorithmic_bytes_per_launch": alg,
+                     # every non-zero gathers one 256-byte row of X (mostly out of L2 at yelp2018 size)
                      "l2_gather": {"bytes_per_launch": 4 * nnzA * CFG["d"], "achieved": 4 * nnzA * CFG["d"] / (spmm_ms * 1e-3) / 1e9,
-                                   "peak": 18500.0, "unit": "GB/s", "frac": 4 * nnzA * CFG["d"] / (spmm_ms * 1e-3) / 1e9 / 18500.0,
-                                   "peak_source": "measured random 256 B row gathers from an L2-resident table, 148 SMs"},
+                                   "unit": "GB/s"},
                      "step": {"algorithmic_bytes": sbytes, "achieved": sbytes / (ms / args.steps * 1e-3) / 1e9,
                               "frac": sbytes / (ms / args.steps * 1e-3) / 1e9 / pk["hbm_gbs"]}},
         "rank": {"metric": "full-catalog rank items/sec", "value": rank_val, "unit": "items/s", "ms": rank_ms,
@@ -841,7 +811,7 @@ def run_sharded(args, rank, world, local_rank):
                                   f"applies the epilogue and stores the finished rows to every rank ({route}), beside the user-side product; 2 synchronisations per "
                                   "layer folded into the kernels; last forward layer on the batch rows only; batch losses replicated on a compact [5B, d] "
                                   "table; one srb_shard_step call per step, captured in a CUDA graph",
-                   "l2": "no flush: per-step working set > 126 MB L2",
+                   "l2": "no flush: per-step working set > 50 MB L2",
                    "inputs": f"{P} pre-sampled batches resident in HBM on every rank; CUDA-graph replay"},
         "clocks": clk,
         "parity": parity, "parity_max_rel": parity_max, "parity_note": "parity_max_rel = the strict (eps = 0) runs; see bench.py run_sharded",
@@ -869,7 +839,14 @@ def main():
     ap.add_argument("--profile", action="store_true", help="eager steps only, for ncu (never a bench value)")
     ap.add_argument("--skip-configs", action="store_true", help="headline metric only (no config2/4/5 sub-records)")
     ap.add_argument("--skip-cpu", action="store_true", help="no cpu_baseline leg")
+    ap.add_argument("--dump-outputs", metavar="DIR", help="write the last timed step's outputs as DIR/<name>.npy (N = 1)")
     args = ap.parse_args()
+    if args.dump_outputs and int(os.environ.get("WORLD_SIZE", "1")) > 1:
+        ap.error("--dump-outputs is supported for the single-GPU run only")
+    if args.dump_outputs and args.impl == "reference":
+        ap.error("--dump-outputs writes the outputs of the GPU path; it does not apply to --impl reference")
+    if args.steps < 1 or args.warmup < 0:
+        ap.error("--steps must be >= 1 and --warmup >= 0")
     claim_stdout()
     rank = int(os.environ.get("RANK", "0"))
     world = int(os.environ.get("WORLD_SIZE", "1"))

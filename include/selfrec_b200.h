@@ -66,7 +66,7 @@ typedef struct srb_hub_split {
   float* part;          /* [n_work, d] scratch (one product at a time per graph) */
   /* Column-blocked variant of the static lists (optional; seg != NULL selects it).  At config-5 size the split rows
    * hold ~40 % of the non-zeros and their gathers miss L2 (the X table is 6 GB): cutting every split row at column-block
-   * boundaries (a block of X rows ~ 32 MB) and processing ALL rows' segments of one block before the next keeps that
+   * boundaries (a block of X rows = a quarter of the L2, 12.5 MB on an H100) and processing ALL rows' segments of one block before the next keeps that
    * block of X in L2, so it is read from HBM once per product instead of once per row.
    *   seg[w] = (begin, end) CSR positions of segment w; a row's segments are consecutive slots (first[r], seg_cnt[r]);
    *   n_work = number of segments (capacity of part);
@@ -328,7 +328,7 @@ typedef struct srb_topk_desc {
   int32_t k;
   int32_t* out_ids;
   float* out_scores;
-  int32_t impl; /* 0 auto; 1 CUDA cores, exact fp32; 2 tcgen05 TF32 candidate lists (2 x 24 per user) + exact fp32
+  int32_t impl; /* 0 auto; 1 CUDA cores, exact fp32; 2 wgmma TF32 candidate lists (2 x 24 per user) + exact fp32
                    rescoring + a per-user exactness certificate, uncertified users re-run by the exact path */
   void* workspace; /* impl 2: srb_topk_workspace_bytes */
   int64_t workspace_bytes;

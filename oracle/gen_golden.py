@@ -1,6 +1,6 @@
-"""Generate tests/golden/*.npz by running the REFERENCE itself (imported from /root/reference).
+"""Generate tests/golden/*.npz by running the REFERENCE itself (imported from a checkout of it).
 
-    python oracle/gen_golden.py [--ref /root/reference] [--out tests/golden]
+    python oracle/gen_golden.py --ref <reference checkout> [--out tests/golden]
 
 The reference has no tests and seeds nothing (SURVEY 4), so the golden vectors are produced
 here: a small synthetic dataset is written in the reference's text format, the reference's
@@ -48,7 +48,7 @@ def make_dataset(rng, n_users=48, n_items=60, n_train=520, n_test=120, dup=3):
 
 def main():
     ap = argparse.ArgumentParser()
-    ap.add_argument("--ref", default="/root/reference")
+    ap.add_argument("--ref", required=True, help="root of a Coder-Yu/SELFRec checkout")
     ap.add_argument("--out", default=os.path.join(os.path.dirname(os.path.abspath(__file__)), "..", "tests", "golden"))
     args = ap.parse_args()
     out = os.path.abspath(args.out)

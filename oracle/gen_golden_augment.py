@@ -1,8 +1,8 @@
 """Golden vectors for R11 (data/augmentor.py): runs the UNMODIFIED reference GraphAugmentor on a fixed matrix with
 fixed `random` seeds and records what it drops.  Test infrastructure; run in the build container only
-(needs /root/reference):
+(needs a checkout of the reference):
 
-    python oracle/gen_golden_augment.py [--ref /root/reference] [--out tests/golden]
+    python oracle/gen_golden_augment.py --ref <reference checkout> [--out tests/golden]
 """
 import argparse
 import os
@@ -15,7 +15,7 @@ import scipy.sparse as sp
 
 def main():
     ap = argparse.ArgumentParser()
-    ap.add_argument("--ref", default="/root/reference")
+    ap.add_argument("--ref", required=True, help="root of a Coder-Yu/SELFRec checkout")
     ap.add_argument("--out", default=os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "tests", "golden"))
     args = ap.parse_args()
     sys.path.insert(0, args.ref)

@@ -3,7 +3,7 @@
 TEST INFRASTRUCTURE / BASELINE ONLY (same rule as oracle.py): used by bench.py's cpu_baseline
 and `--impl reference` legs and by tests; never by the product.
 
-/root/reference cannot travel to the GPU box (and is not pip-installable: no setup.py), so the
+The reference cannot ship with this repository (and is not pip-installable: no setup.py), so the
 "reference arm" is this port: the same torch ops the reference calls, in the same order, on
 the host cores (torch.set_num_threads(os.cpu_count())), driven by the same Python sampler
 algorithm.  tests/test_oracle_golden.py pins it against the reference-generated fixtures.

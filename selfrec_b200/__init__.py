@@ -1,4 +1,4 @@
-"""selfrec_b200: the B200-native hot path behind SELFRec's plugin surface.
+"""selfrec_b200: the H100-native hot path behind SELFRec's plugin surface.
 
     import selfrec_b200
     selfrec_b200.install()          # alias base.*, util.*, data.*, model.graph.* in sys.modules

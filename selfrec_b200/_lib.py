@@ -230,7 +230,7 @@ def require_device():
     """Raise unless a CUDA device is usable (no CPU fallback)."""
     lib = load()
     if lib.srb_device_ok() != 0:
-        raise SrbError("selfrec_b200 needs a CUDA device (sm_100a): " + last_error())
+        raise SrbError("selfrec_b200 needs a CUDA device (sm_90a): " + last_error())
     return lib
 
 

@@ -2,7 +2,7 @@
 
 convert_sparse_mat_to_tensor returns a SparseAdj handle instead of a torch COO tensor: the
 callers' `.cuda()` uploads the CSR once and `torch.sparse.mm(handle, dense)` dispatches to
-the sm_100a SpMM kernel (differentiable w.r.t. the dense operand)."""
+the sm_90a SpMM kernel (differentiable w.r.t. the dense operand)."""
 from ..ops import SparseAdj
 
 

@@ -1,4 +1,4 @@
-"""Build libselfrec_b200.so (CUDA kernels + C ABI) in-tree with nvcc for sm_100a.
+"""Build libselfrec_b200.so (CUDA kernels + C ABI) in-tree with nvcc for sm_90a (H100).
 
     python -m selfrec_b200.build [--force] [--verbose]
 
@@ -21,11 +21,10 @@ STAMP = os.path.join(HERE, "libselfrec_b200.stamp")  # no leading dot: it has to
 LOCK = os.path.join(HERE, "libselfrec_b200.lock")
 
 SOURCES = ["capi.cu", "spmm.cu", "bpr.cu", "infonce.cu", "score_topk.cu", "score_topk_tc.cu", "engine.cu", "sharded.cu", "graphbuild.cu", "sampler.cpp", "dataset.cpp"]
-NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a",
+ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]
+NVCC_FLAGS = ARCH + [
     "-O3", "-std=c++17", "-lineinfo",
     "-Xcompiler", "-fPIC,-O3,-Wall",
-    "--shared",
 ]
 
 
@@ -55,7 +54,7 @@ def needs_build():
 
 
 def build(force=False, verbose=False):
-    """Compile every CUDA source for sm_100a into selfrec_b200/libselfrec_b200.so."""
+    """Compile every CUDA source for sm_90a into selfrec_b200/libselfrec_b200.so."""
     if not force and not needs_build():
         return LIB
     # several ranks of one job may get here at once: one builds, the others wait and find it done
@@ -78,8 +77,7 @@ def _build_locked(verbose):
     for src in SOURCES:
         obj = os.path.join(objdir, src.rsplit(".", 1)[0] + ".o")
         objs.append(obj)
-        cmd = [nvcc, "-gencode", "arch=compute_100a,code=sm_100a", "-O3", "-std=c++17", "-lineinfo",
-               "-Xcompiler", "-fPIC,-O3,-Wall", "-I", INCLUDE, "-I", CSRC, "-c", os.path.join(CSRC, src), "-o", obj]
+        cmd = [nvcc] + NVCC_FLAGS + ["-I", INCLUDE, "-I", CSRC, "-c", os.path.join(CSRC, src), "-o", obj]
         if verbose:
             cmd.insert(1, "-Xptxas=-v")
         procs.append((src, subprocess.Popen(cmd, stdout=subprocess.PIPE, stderr=subprocess.STDOUT, text=True)))
@@ -94,7 +92,7 @@ def _build_locked(verbose):
     if failed:
         raise RuntimeError("nvcc failed; see messages above")
     tmp = LIB + f".tmp{os.getpid()}"
-    link = [nvcc, "--shared", "-gencode", "arch=compute_100a,code=sm_100a", "-o", tmp] + objs
+    link = [nvcc, "--shared"] + ARCH + ["-o", tmp] + objs
     r = subprocess.run(link, stdout=subprocess.PIPE, stderr=subprocess.STDOUT, text=True)
     if r.returncode != 0:
         raise RuntimeError("link failed:\n" + r.stdout)

@@ -22,7 +22,19 @@ int sm_count() {
     if (cudaGetDevice(&dev) == cudaSuccess && cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) == cudaSuccess && n > 0)
       cached = n;
     else
-      cached = 148;  // B200
+      cached = 132;  // H100 SXM
+  }
+  return cached;
+}
+
+long long l2_bytes() {
+  static long long cached = 0;
+  if (cached == 0) {
+    int dev = 0, n = 0;
+    if (cudaGetDevice(&dev) == cudaSuccess && cudaDeviceGetAttribute(&n, cudaDevAttrL2CacheSize, dev) == cudaSuccess && n > 0)
+      cached = n;
+    else
+      cached = 50ll << 20;  // H100
   }
   return cached;
 }

@@ -1,4 +1,4 @@
-// Shared helpers for the selfrec_b200 kernels (sm_100a only).
+// Shared helpers for the selfrec_b200 kernels (sm_90a only).
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -42,6 +42,7 @@ inline int post_launch(const char* what) {
   } while (0)
 
 int sm_count();
+long long l2_bytes();  // L2 size of the current device
 
 // sparse-row scatter with several (src, rows) segments in one launch (bpr.cu)
 struct ScatterSeg {

@@ -134,7 +134,8 @@ __global__ void __launch_bounds__(256) nce_prep_kernel(const NceArgs a) {
 
 // Tensor-core pipeline (d = 64): gather + normalise 32 rows per CTA; besides the exact rows it writes the
 // TF32 hi / lo parts (x = hi + lo, hi = rna_tf32(x); the tensor core truncates lo) of both views, row-major
-// and transposed (through shared memory, so the transposed stores are 128-byte coalesced), behind dV2:
+// and transposed (through shared memory, so the transposed stores are 128-byte coalesced; columns in the
+// nce_tperm order the tensor-core kernel expects), behind dV2:
 //   hi: [V1 | V2 | V1^T | V2^T]   then lo: the same four
 __global__ void __launch_bounds__(256) nce_prep_tc_kernel(const NceArgs a) {
   constexpr int D = 64;
@@ -189,7 +190,7 @@ __global__ void __launch_bounds__(256) nce_prep_tc_kernel(const NceArgs a) {
   __syncthreads();
   for (int e = threadIdx.x; e < D * 32; e += 256) {
     const int dc = e >> 5, il = e & 31;
-    const size_t o = (size_t)dc * a.np + i0 + il;
+    const size_t o = (size_t)dc * a.np + i0 + nce_tperm(il);  // columns permuted within groups of 8 (infonce_tc.cuh)
     const float x1 = t1[il][dc], x2 = t2[il][dc];
     const float g1 = tf32_rna(x1), g2 = tf32_rna(x2);
     hi[2 * nd + o] = g1;
@@ -544,7 +545,7 @@ static int nce_launch_tc(const NceArgs& a, int n_problems, cudaStream_t st) {
   t.np = np;
   t.inv_tau = a.inv_tau;
   const int row_blocks = np / NT_T;
-  // one CTA per SM (224 KB of shared memory each): as many column splits as fit in a single wave
+  // one CTA per SM (193 KB of shared memory each): as many column splits as fit in a single wave
   int splits = sm_count() / (row_blocks * n_problems);
   if (splits < 1) splits = 1;
   if (splits > NT_MAX_SPLITS) splits = NT_MAX_SPLITS;

@@ -1,7 +1,7 @@
-// (iii) InfoNCE forward/backward on the 5th-gen tensor cores (tcgen05, TF32), d = 64.
+// (iii) InfoNCE forward/backward on the Hopper tensor cores (wgmma, TF32), d = 64.
 //
 // Same contract as infonce.cu (util/loss_torch.py:35-50 + autograd backward); the n x n logit matrix
-// lives only in TMEM / shared memory.  Per problem, with V1, V2 the L2-normalised gathered views:
+// lives only in registers.  Per problem, with V1, V2 the L2-normalised gathered views:
 //   pass A  rows = view-1 rows i:  E = exp(S - 1/tau)  (|S| <= 1/tau: cosines, so the shift needs no running max);
 //           l_i += sum_j E_ij (the softmax denominator) and, unnormalised, dV1_i += sum_{j != i} E_ij V2_j
 //           -- forward (LSE) and the view-1 gradient in ONE sweep: the 1/l_i factor is applied afterwards
@@ -9,18 +9,18 @@
 //   finish  scales dV1 by w/(n tau l_i), adds the diagonal term (P_ii - 1) w/(n tau) v_i in exact fp32, then the
 //           normalisation backward
 // Each CTA owns a block of 128 rows and a strided subset of the 64-column tiles:
-//   warp 0    TMA producer: column-operand tile [64 x 64] (K-major over d, for S; 3-stage ring) and, for the
-//             GRAD passes, the same tile from the transposed copy [64 d x 64 cols] (K-major over the
-//             column index, for G V; 2-stage ring), 128-byte swizzle
-//   warp 1    MMA issuer:   S[128 x 64]  = A B^T           M=128 N=64, 8 k-steps x 3 products, operands in smem
-//                           D[128 x 64] += G[128 x 64] Vt^T same shape, the G operand read from TENSOR MEMORY
-//   warps 2-9 epilogue:     thread = (row, 32-column half).  tcgen05.ld the S chunk -> G chunk in registers
-//                           (one FFMA + MUFU.EX2 + one conversion per element) -> tcgen05.st into the
-//                           double-buffered G region of tensor memory -> hand it to the MMA warp;
-//                           finally D -> global (red.v4 over splits)
-// Tensor memory (512 columns): S stage 0 | S stage 1 | D | G0 hi | G0 lo | G1 hi | G1 lo, 64 columns each.
-// An MN-major B operand would let one tile serve both products, but tcgen05.mma kind::tf32 with the
-// b_major bit set returns zeros on this hardware (tools/tc_probe.cu variants 2-7), hence the transposed copy.
+//   warp 8        TMA producer: per tile, the column operand [64 x 64] (K-major over d, for S) and the same tile
+//                 from the transposed copy [64 d x 64 cols] (K-major over the column index, for G V), hi and lo
+//                 parts, 128-byte swizzle, 2-stage ring
+//   warpgroups 0, 1 (64 rows each):
+//                 S[64 x 64]  = A B^T         wgmma m64n64k8, 8 k-steps x 3 products, operands in smem
+//                 G = exp(...) in registers, split into TF32 hi / lo
+//                 D[64 x 64] += G Vt^T        same shape, the G operand taken straight from the registers that
+//                                             held S; finally D -> global (red.v2 over splits)
+// The accumulator fragment of S holds columns 2t, 2t+1 of every 8-column k-step where the register A fragment
+// of the next product wants columns t, t+4.  Instead of shuffling, the transposed copy is written with the columns
+// of every group of 8 permuted (column o stored at position (o >> 1) + 4 (o & 1), nce_tperm), so that the k-step's
+// B rows match the A fragment as it stands.
 // fp32 accuracy on a TF32 pipe: every operand is split x = hi + lo (hi = rna_tf32(x), lo = x - hi, which
 // the tensor core truncates to TF32) and each product is evaluated as hi*hi + hi*lo + lo*hi ("3xTF32",
 // error ~2^-21 instead of 2^-11).  S_ii and the normalisation backward use the exact fp32 rows.
@@ -33,23 +33,24 @@ namespace srb {
 using namespace tc;
 
 constexpr int NT_D = 64;
-constexpr int NT_T = 128;        // rows per CTA (UMMA M)
-constexpr int NT_C = 64;         // columns per tile (UMMA N of the S product, K of the G V product)
-constexpr int NT_STAGES = 3;
-constexpr int NT_EPI_WARPS = 8;
-constexpr int NT_THREADS = 64 + 32 * NT_EPI_WARPS;  // warp 0 TMA, warp 1 MMA, warps 2..9 epilogue
+constexpr int NT_T = 128;        // rows per CTA (two warpgroups of wgmma M = 64)
+constexpr int NT_C = 64;         // columns per tile (wgmma N of the S product, K of the G V product)
+constexpr int NT_STAGES = 2;
+constexpr int NT_THREADS = 256 + 32;  // warpgroups 0-1 MMA + exponentials, warp 8 TMA
 constexpr int NT_MAX_SPLITS = 8;
 constexpr uint32_t NT_ATILE = NT_T * NT_D * 4;   // 32 KB: 2 k-chunks x [128][32]      (x2: hi, lo)
 constexpr uint32_t NT_BTILE = NT_C * NT_D * 4;   // 16 KB: 2 k-chunks x [64][32]       (x2: hi, lo)
 constexpr uint32_t NT_TTILE = NT_D * NT_C * 4;   // 16 KB: 2 column chunks x [64][32]  (x2: hi, lo)
-constexpr int NT_TSTAGES = 2;
+constexpr uint32_t NT_STAGE = 2 * NT_BTILE + 2 * NT_TTILE;  // one ring stage: B hi | B lo | Bt hi | Bt lo
+
+// position of column i of a 64-column tile in the transposed copies (see above)
+__host__ __device__ __forceinline__ int nce_tperm(int i) { return (i & ~7) | (((i & 7) >> 1) + 4 * (i & 1)); }
 
 struct NtSmem {
   static constexpr uint32_t a_off = 0;                                  // row-operand tile hi|lo (fixed per CTA)  64 KB
-  static constexpr uint32_t b_off = a_off + 2 * NT_ATILE;               // 3 stages x (hi|lo) column tile          96 KB
-  static constexpr uint32_t bt_off = b_off + NT_STAGES * 2 * NT_BTILE;  // 2 stages x (hi|lo) transposed tile      64 KB
-  static constexpr uint32_t bar_off = bt_off + NT_TSTAGES * 2 * NT_TTILE;
-  static constexpr uint32_t total = bar_off + 1024;                     // barriers + column constants (GRAD-B)
+  static constexpr uint32_t b_off = a_off + 2 * NT_ATILE;               // 2 stages x (B hi|lo, Bt hi|lo)        128 KB
+  static constexpr uint32_t bar_off = b_off + NT_STAGES * NT_STAGE;
+  static constexpr uint32_t total = bar_off + 1024;                     // barriers + column constants (pass B)
 };
 
 struct NtProblem {
@@ -96,18 +97,10 @@ __global__ void __launch_bounds__(NT_THREADS, 1) nce_tc_kernel(const __grid_cons
   extern __shared__ __align__(1024) uint8_t nt_smem_raw[];
   uint8_t* sm = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(nt_smem_raw) + 1023) & ~(uintptr_t)1023);
   uint64_t* bars = reinterpret_cast<uint64_t*>(sm + NtSmem::bar_off);
-  uint64_t* bar_full = bars;          // [3] TMA -> MMA (column tiles)
-  uint64_t* bar_empty = bars + 3;     // [3] last product that reads the stage done -> TMA
-  uint64_t* bar_sfull = bars + 6;     // [2] S accumulator ready -> epilogue
-  uint64_t* bar_sempty = bars + 8;    // [2] epilogue drained S -> MMA
-  uint64_t* bar_gfull = bars + 10;    // [2] G tile written to tensor memory -> MMA
-  uint64_t* bar_gempty = bars + 12;   // [2] G V product consumed G -> epilogue
-  uint64_t* bar_tfull = bars + 14;    // [2] TMA -> MMA (transposed tiles)
-  uint64_t* bar_tempty = bars + 16;   // [2] G V product done -> TMA
-  uint64_t* bar_a = bars + 18;        // [1] row tile loaded
-  uint64_t* bar_dfull = bars + 19;    // [1] final D accumulator ready
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 20);
-  float* colc = reinterpret_cast<float*>(bars + 24);  // [2][64] GRAD-B: per-column exponent offsets, double-buffered
+  uint64_t* bar_full = bars;                // [2] TMA -> MMA (column tiles, both layouts)
+  uint64_t* bar_empty = bars + NT_STAGES;   // [2] both warpgroups' G V products done -> TMA
+  uint64_t* bar_a = bars + 2 * NT_STAGES;   // [1] row tile loaded
+  float* colc = reinterpret_cast<float*>(bars + 8);  // [2][64] pass B: per-column exponent offsets, double-buffered
 
   const int prob = blockIdx.z;
   const NtProblem& P = a.p[prob];
@@ -127,32 +120,14 @@ __global__ void __launch_bounds__(NT_THREADS, 1) nce_tc_kernel(const __grid_cons
   if (threadIdx.x == 0) {
     for (int s = 0; s < NT_STAGES; ++s) {
       mbar_init(bar_full + s, 1);
-      mbar_init(bar_empty + s, 1);
-    }
-    for (int s = 0; s < 2; ++s) {
-      mbar_init(bar_sfull + s, 1);
-      mbar_init(bar_sempty + s, NT_EPI_WARPS);
-      mbar_init(bar_gfull + s, NT_EPI_WARPS);
-      mbar_init(bar_gempty + s, 1);
-      mbar_init(bar_tfull + s, 1);
-      mbar_init(bar_tempty + s, 1);
+      mbar_init(bar_empty + s, 2);  // one arrive per consumer warpgroup
     }
     mbar_init(bar_a, 1);
-    mbar_init(bar_dfull, 1);
     fence_barrier_init();
   }
-  if (warp == 1) {
-    tmem_alloc(tmem_slot, 512);
-    tmem_relinquish();
-  }
-  fence_before_sync();
   __syncthreads();
-  fence_after_sync();
-  const uint32_t tmem = *tmem_slot;
-  const uint32_t tmem_d = tmem + 128;  // columns [128, 192): the G V accumulator; S stages at [0,64), [64,128)
-  const uint32_t tmem_g = tmem + 192;  // G buffers: [192 + 128 b, +64) hi, [+64, +128) lo
 
-  if (warp == 0) {
+  if (warp == 8) {
     if (elect_one()) {
       mbar_arrive_expect_tx(bar_a, 2 * NT_ATILE);
       for (int h = 0; h < 2; ++h)
@@ -160,186 +135,133 @@ __global__ void __launch_bounds__(NT_THREADS, 1) nce_tc_kernel(const __grid_cons
       for (int k = 0; k < my_tiles; ++k) {
         const int t = split + k * a.splits;
         const int s = k % NT_STAGES;
+        uint8_t* st = sm + NtSmem::b_off + s * NT_STAGE;
         mbar_wait(bar_empty + s, ((k / NT_STAGES) & 1) ^ 1);
-        mbar_arrive_expect_tx(bar_full + s, 2 * NT_BTILE);
+        mbar_arrive_expect_tx(bar_full + s, NT_STAGE);
         for (int h = 0; h < 2; ++h)
-          for (int c = 0; c < 2; ++c)
-            tma_load_2d(sm + NtSmem::b_off + (s * 2 + h) * NT_BTILE + c * 8192, &map_col[h], bar_full + s, c * 32, t * NT_C);
-        {
-          const int ts = k & 1;
-          mbar_wait(bar_tempty + ts, ((k >> 1) & 1) ^ 1);
-          mbar_arrive_expect_tx(bar_tfull + ts, 2 * NT_TTILE);
-          for (int h = 0; h < 2; ++h)
-            for (int c = 0; c < 2; ++c)
-              tma_load_2d(sm + NtSmem::bt_off + (ts * 2 + h) * NT_TTILE + c * 8192, &map_colt[h], bar_tfull + ts, t * NT_C + c * 32, 0);
-        }
-      }
-    }
-  } else if (warp == 1) {
-    if (elect_one()) {
-      const uint32_t idesc = make_idesc_tf32(128, NT_C);   // both products: M = 128, N = 64
-      const uint32_t a_base = smem_u32(sm + NtSmem::a_off);
-      mbar_wait(bar_a, 0);
-      auto issue_s = [&](int k) {
-        const int s = k & 1;
-        const int sb = k % NT_STAGES;
-        mbar_wait(bar_sempty + s, ((k >> 1) & 1) ^ 1);
-        mbar_wait(bar_full + sb, (k / NT_STAGES) & 1);
-        fence_after_sync();
-        const uint32_t b_base = smem_u32(sm + NtSmem::b_off + sb * 2 * NT_BTILE);
-        // S = Ahi Bhi + Ahi Blo + Alo Bhi
-#pragma unroll
-        for (int pr = 0; pr < 3; ++pr) {
-          const uint32_t ab = a_base + (pr == 2 ? NT_ATILE : 0);
-          const uint32_t bb = b_base + (pr == 1 ? NT_BTILE : 0);
-#pragma unroll
-          for (int c = 0; c < 2; ++c)
-#pragma unroll
-            for (int kk = 0; kk < 4; ++kk)
-              umma_tf32_ss(tmem + s * 64, make_smem_desc_k_sw128(ab + c * 16384 + kk * 32),
-                           make_smem_desc_k_sw128(bb + c * 8192 + kk * 32), idesc, (pr | c | kk) ? 1u : 0u);
-        }
-        umma_commit(bar_sfull + s);
-        umma_commit(bar_empty + sb);  // the column tile (K-major copy) is free once S is computed
-      };
-      issue_s(0);
-      for (int k = 0; k < my_tiles; ++k) {
-        if (k + 1 < my_tiles) issue_s(k + 1);  // S of the next tile overlaps the epilogue of this one
-        {
-          const int gs = k & 1;
-          const uint32_t bt_base = smem_u32(sm + NtSmem::bt_off + gs * 2 * NT_TTILE);
-          const uint32_t g_hi = tmem_g + gs * 128;
-          mbar_wait(bar_gfull + gs, (k >> 1) & 1);
-          mbar_wait(bar_tfull + gs, (k >> 1) & 1);
-          fence_after_sync();
-          // D += Ghi Vhi + Glo Vhi + Ghi Vlo      (K = the 64 columns of this tile, 8 per MMA; G from tensor memory)
-#pragma unroll
-          for (int pr = 0; pr < 3; ++pr) {
-            const uint32_t ga = g_hi + (pr == 1 ? 64 : 0);
-            const uint32_t vb = bt_base + (pr == 2 ? NT_TTILE : 0);
-#pragma unroll
-            for (int kk = 0; kk < 8; ++kk)
-              umma_tf32_ts(tmem_d, ga + kk * 8, make_smem_desc_k_sw128(vb + (kk >> 2) * 8192 + (kk & 3) * 32), idesc,
-                           (k | pr | kk) ? 1u : 0u);
+          for (int c = 0; c < 2; ++c) {
+            tma_load_2d(st + h * NT_BTILE + c * 8192, &map_col[h], bar_full + s, c * 32, t * NT_C);
+            tma_load_2d(st + 2 * NT_BTILE + h * NT_TTILE + c * 8192, &map_colt[h], bar_full + s, t * NT_C + c * 32, 0);
           }
-          umma_commit(bar_gempty + gs);  // G buffer reusable
-          umma_commit(bar_tempty + gs);  // transposed tile reusable
-        }
-      }
-      umma_commit(bar_dfull);
-    }
-  } else {
-    // ===== epilogue warps: thread = one row of the block x one 32-column half of the tile =====
-    const int quarter = warp & 3;          // TMEM lane quarter this warp may read
-    const int half = (warp - 2) >> 2;      // column chunk [32*half, 32*half + 32) of each tile
-    const int et = threadIdx.x - 64;       // 0..255
-    const int row_l = quarter * 32 + lane;
-    const int row = r0 + row_l;
-    const bool row_ok = row < n;
-    const float L2E = 1.4426950408889634f;
-    const float sc = a.inv_tau * L2E;      // exponent scale: 2^(s*sc + off) = e^(s/tau + off/log2(e))
-    const float gscale = P.weight * a.inv_tau / (float)n;
-    const float lg = log2f(gscale);
-    float l_run = 0.f;  // pass A: sum of exp(S - 1/tau) over my columns
-    // pass B: exponent offset of column c = log2(w/(n tau)) - lse_c log2(e), lse_c = 1/tau + ln l_c; the CTAs of the
-    // first row block see every column exactly once and also accumulate the loss = mean(lse_i - S_ii), S_ii exact
-    auto col_const = [&](int col) -> float {
-      float off = -INFINITY, contrib = 0.f;
-      if (col < n) {
-        const float lse = a.inv_tau + logf(P.lsum[col]);
-        off = lg - lse * L2E;
-        contrib = lse - P.diag[col];
-      }
-      if (blockIdx.x == 0) {
-        contrib = warp_sum(contrib);
-        if (lane == 0) atomicAdd(P.loss_acc, contrib);
-      }
-      return off;
-    };
-    float next_colc = 0.f;
-    if (MODE == 2) {  // column constants of tile 0
-      if (et < NT_C) colc[et] = col_const(split * NT_C + et);
-      asm volatile("bar.sync 1, 256;" ::: "memory");
-    }
-    for (int k = 0; k < my_tiles; ++k) {
-      const int t = split + k * a.splits;
-      const int s = k & 1;
-      const int cb = t * NT_C + half * 32;  // first column of my chunk
-      if (MODE == 2 && et < NT_C && k + 1 < my_tiles) next_colc = col_const((t + a.splits) * NT_C + et);  // prefetch
-      mbar_wait(bar_sfull + s, (k >> 1) & 1);
-      fence_after_sync();
-      uint32_t r[32];
-      tmem_ld_32x32(tmem + ((uint32_t)(quarter * 32) << 16) + s * 64 + half * 32, r);
-      tmem_ld_wait();
-      fence_before_sync();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(bar_sempty + s);  // S stage drained (values are in registers)
-      {
-        // G chunk: pass A x = exp(s/tau - 1/tau), pass B x = exp(s/tau - lse_col) * w/(n tau).  The diagonal term
-        // (P_ii - 1) v_i is added in exact fp32 by the finish kernel: through the tensor core its TF32 rounding
-        // (|G_ii| ~ 1) would dominate the row.  Rows >= n only reach rows >= n of D, which are never written.
-        uint32_t lo[32];
-        const float* cc = colc + (k & 1) * NT_C + half * 32;
-        const bool edge = (MODE == 1 && cb + 32 > n) || (row >= cb && row < cb + 32);
-        if (!edge) {
-#pragma unroll
-          for (int j = 0; j < 32; ++j) {
-            const float off = (MODE == 1) ? -sc : cc[j];
-            const float x = ex2_approx(fmaf(__uint_as_float(r[j]), sc, off));
-            if (MODE == 1) l_run += x;
-            const float h = to_tf32_rna(x);
-            r[j] = __float_as_uint(h);
-            lo[j] = __float_as_uint(x - h);
-          }
-        } else {
-#pragma unroll
-          for (int j = 0; j < 32; ++j) {
-            const float off = (MODE == 1) ? -sc : cc[j];
-            float x = ex2_approx(fmaf(__uint_as_float(r[j]), sc, off));
-            if (cb + j >= n) x = 0.f;
-            if (MODE == 1) l_run += x;  // the denominator includes the diagonal
-            if (cb + j == row) x = 0.f;
-            const float h = to_tf32_rna(x);
-            r[j] = __float_as_uint(h);
-            lo[j] = __float_as_uint(x - h);
-          }
-        }
-        const int gs = k & 1;
-        mbar_wait(bar_gempty + gs, ((k >> 1) & 1) ^ 1);  // G buffer consumed by the tensor core two tiles ago
-        fence_after_sync();
-        const uint32_t gaddr = tmem_g + gs * 128 + ((uint32_t)(quarter * 32) << 16) + half * 32;
-        tmem_st_32x32(gaddr, r);
-        tmem_st_32x32(gaddr + 64, lo);
-        tmem_st_wait();
-        fence_before_sync();
-        __syncwarp();
-        if (lane == 0) mbar_arrive(bar_gfull + gs);
-        if (MODE == 2) {
-          if (et < NT_C && k + 1 < my_tiles) colc[((k + 1) & 1) * NT_C + et] = next_colc;
-          asm volatile("bar.sync 1, 256;" ::: "memory");
-        }
       }
     }
-    {
-      if (MODE == 1 && row_ok) atomicAdd(P.lsum + row, l_run);
-      mbar_wait(bar_dfull, 0);
-      fence_after_sync();
-      float* out = ((MODE == 1) ? P.dV1 : P.dV2) + (size_t)row * NT_D + half * 32;
-      uint32_t r[32];
-      tmem_ld_32x32(tmem_d + ((uint32_t)(quarter * 32) << 16) + half * 32, r);
-      tmem_ld_wait();
-      if (row_ok) {
+    return;
+  }
+  // ===== consumer warpgroup wg: rows r0 + 64 wg .. +63 =====
+  const int wg = warp >> 2;
+  const int w4 = warp & 3, g = lane >> 2, tq = lane & 3;
+  const int et = threadIdx.x;            // 0..255
+  const int row_a = r0 + wg * 64 + w4 * 16 + g;  // accumulator rows of this thread: row_a, row_a + 8
+  const float L2E = 1.4426950408889634f;
+  const float sc = a.inv_tau * L2E;      // exponent scale: 2^(s*sc + off) = e^(s/tau + off/log2(e))
+  const float gscale = P.weight * a.inv_tau / (float)n;
+  const float lg = log2f(gscale);
+  float l_run[2] = {0.f, 0.f};  // pass A: sum of exp(S - 1/tau) over my columns, rows row_a and row_a + 8
+  // pass B: exponent offset of column c = log2(w/(n tau)) - lse_c log2(e), lse_c = 1/tau + ln l_c; the CTAs of the
+  // first row block see every column exactly once and also accumulate the loss = mean(lse_i - S_ii), S_ii exact
+  auto col_const = [&](int col) -> float {
+    float off = -INFINITY, contrib = 0.f;
+    if (col < n) {
+      const float lse = a.inv_tau + logf(P.lsum[col]);
+      off = lg - lse * L2E;
+      contrib = lse - P.diag[col];
+    }
+    if (blockIdx.x == 0) {
+      contrib = warp_sum(contrib);
+      if (lane == 0) atomicAdd(P.loss_acc, contrib);
+    }
+    return off;
+  };
+  float next_colc = 0.f;
+  if (MODE == 2) {  // column constants of tile 0
+    if (et < NT_C) colc[et] = col_const(split * NT_C + et);
+    named_bar_sync(1, 256);
+  }
+  const uint32_t a_base = smem_u32(sm + NtSmem::a_off + wg * 8192);
+  float d[32];
 #pragma unroll
-        for (int u = 0; u < 8; ++u)
-          atomicAdd(reinterpret_cast<float4*>(out + 4 * u),
-                    make_float4(__uint_as_float(r[4 * u]), __uint_as_float(r[4 * u + 1]), __uint_as_float(r[4 * u + 2]),
-                                __uint_as_float(r[4 * u + 3])));  // red.global.add.v4.f32
+  for (int j = 0; j < 32; ++j) d[j] = 0.f;
+  mbar_wait(bar_a, 0);
+  for (int k = 0; k < my_tiles; ++k) {
+    const int t = split + k * a.splits;
+    const int s = k % NT_STAGES;
+    const int cb = t * NT_C;  // first column of the tile
+    if (MODE == 2 && et < NT_C && k + 1 < my_tiles) next_colc = col_const((t + a.splits) * NT_C + et);  // prefetch
+    mbar_wait(bar_full + s, (k / NT_STAGES) & 1);
+    const uint32_t b_base = smem_u32(sm + NtSmem::b_off + s * NT_STAGE);
+    // S = Ahi Bhi + Ahi Blo + Alo Bhi
+    float sv[32];
+    wgmma_fence();
+#pragma unroll
+    for (int pr = 0; pr < 3; ++pr) {
+      const uint32_t ab = a_base + (pr == 2 ? NT_ATILE : 0);
+      const uint32_t bb = b_base + (pr == 1 ? NT_BTILE : 0);
+#pragma unroll
+      for (int c = 0; c < 2; ++c)
+#pragma unroll
+        for (int kk = 0; kk < 4; ++kk)
+          wgmma_m64n64k8_tf32_ss(sv, make_smem_desc_k_sw128(ab + c * 16384 + kk * 32), make_smem_desc_k_sw128(bb + c * 8192 + kk * 32),
+                                 (pr | c | kk) ? 1u : 0u);
+    }
+    wgmma_commit();
+    wgmma_wait<0>();
+    // G: pass A x = exp(s/tau - 1/tau), pass B x = exp(s/tau - lse_col) * w/(n tau).  The diagonal term
+    // (P_ii - 1) v_i is added in exact fp32 by the finish kernel: through the tensor core its TF32 rounding
+    // (|G_ii| ~ 1) would dominate the row.  Rows >= n only reach rows >= n of D, which are never written.
+    uint32_t hi[32], lo[32];
+    const float* cc = colc + (k & 1) * NT_C;
+    // (selects, not branches: a divergent path between the wgmma groups would serialise them)
+#pragma unroll
+    for (int j = 0; j < 32; ++j) {
+      const int cl = 8 * (j >> 2) + 2 * tq + (j & 1);  // column within the tile
+      const int rh = (j >> 1) & 1;                     // row_a or row_a + 8
+      const float off = (MODE == 1) ? -sc : cc[cl];    // pass B: -inf for columns >= n
+      float x = ex2_approx(fmaf(sv[j], sc, off));
+      if (MODE == 1) {
+        x = (cb + cl < n) ? x : 0.f;
+        l_run[rh] += x;  // the denominator includes the diagonal
       }
+      x = (cb + cl == row_a + 8 * rh) ? 0.f : x;
+      const float h = to_tf32_rna(x);
+      hi[j] = __float_as_uint(h);
+      lo[j] = __float_as_uint(x - h);
+    }
+    // D += Ghi Vhi + Glo Vhi + Ghi Vlo      (K = the 64 columns of this tile, 8 per MMA; G from registers)
+    const uint32_t bt_base = b_base + 2 * NT_BTILE;
+    wgmma_fence();
+#pragma unroll
+    for (int pr = 0; pr < 3; ++pr) {
+      const uint32_t (&ga)[32] = (pr == 1) ? lo : hi;
+      const uint32_t vb = bt_base + (pr == 2 ? NT_TTILE : 0);
+#pragma unroll
+      for (int kk = 0; kk < 8; ++kk)
+        wgmma_m64n64k8_tf32_rs(d, ga[4 * kk], ga[4 * kk + 2], ga[4 * kk + 1], ga[4 * kk + 3],
+                               make_smem_desc_k_sw128(vb + (kk >> 2) * 8192 + (kk & 3) * 32), 1u);
+    }
+    wgmma_commit();
+    wgmma_wait<0>();
+    if ((threadIdx.x & 127) == 0) mbar_arrive(bar_empty + s);  // this warpgroup is done with the stage
+    if (MODE == 2) {
+      if (et < NT_C && k + 1 < my_tiles) colc[((k + 1) & 1) * NT_C + et] = next_colc;
+      named_bar_sync(1, 256);
     }
   }
-  fence_before_sync();
-  __syncthreads();
-  if (warp == 1) tmem_dealloc(tmem, 512);
+#pragma unroll
+  for (int rh = 0; rh < 2; ++rh) {
+    const int row = row_a + 8 * rh;
+    if (MODE == 1) {
+      float l = l_run[rh];
+      l += __shfl_xor_sync(SRB_FULL_MASK, l, 1);
+      l += __shfl_xor_sync(SRB_FULL_MASK, l, 2);
+      if (tq == 0 && row < n) atomicAdd(P.lsum + row, l);
+    }
+    if (row < n) {
+      float* out = ((MODE == 1) ? P.dV1 : P.dV2) + (size_t)row * NT_D;
+#pragma unroll
+      for (int cg = 0; cg < 8; ++cg)  // red.global.add.v2.f32
+        atomicAdd(reinterpret_cast<float2*>(out + 8 * cg + 2 * tq), make_float2(d[4 * cg + 2 * rh], d[4 * cg + 2 * rh + 1]));
+    }
+  }
 }
 
 }  // namespace srb

@@ -245,7 +245,7 @@ static int launch_topk(const TopkArgs& a, cudaStream_t st) {
 
 // ---- fallback of impl 2: exact re-run of the users it could not certify (device-side list) ----
 // Fast path for the first `cap` of them: exact score rows spread over many CTAs + one warp per user
-// for the sequential top-k (a handful of users must not cost a full impl-1 block pass, ~1.6 ms).
+// for the sequential top-k (a handful of users must not cost a full impl-1 pass over the catalogue).
 template <int D>
 __global__ void __launch_bounds__(256) fb_score_kernel(const float* __restrict__ user_emb, const float* __restrict__ item_emb,
                                                       const int32_t* __restrict__ fb_users, const int32_t* __restrict__ fb_count,

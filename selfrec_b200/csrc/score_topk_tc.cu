@@ -1,4 +1,4 @@
-// (iv) impl 2: full-catalog scoring on the 5th-gen tensor cores (tcgen05, TF32) with fused
+// (iv) impl 2: full-catalog scoring on the Hopper tensor cores (wgmma, TF32) with fused
 // rated-item mask + candidate selection, followed by exact fp32 re-scoring.
 //
 // Replaces GraphRecommender.test() base/graph_recommender.py:38-58 (predict XSimGCL.py:57-60,
@@ -6,16 +6,13 @@
 //
 // Stage 1  tc_gather_kernel     users[q] rows -> contiguous [n_q, d] table (TMA cannot gather),
 //                               ||u_q||, max_i ||item_i||
-// Stage 2  tc_score_kernel      one persistent CTA per block of UB <= 256 users, streaming the whole
-//                               catalogue in tiles of 128 items:
-//            warp 0   TMA producer: item tiles [128 x 64] fp32, 128B-swizzled, 3-stage mbarrier ring
-//            warp 1   MMA issuer : tcgen05.mma kind::tf32, M=128 (users) x N=128 (items) x K=8,
-//                                  2 user halves x 8 k-steps per tile, accumulators in TMEM
-//                                  (2 stages x 2 halves x 128 columns = all 512 columns)
-//            warps 2-17 epilogue : 16 warps (4 per scheduler: the select loop is latency-bound), thread =
-//                                  one user row x one 64-column half of the tile: tcgen05.ld (lane = user
-//                                  row), rated-item cursor, per-thread top-24 candidate list (3 buckets
-//                                  of 8, minima in registers) in shared memory -> 2 x 24 candidates per user
+// Stage 2  tc_score_kernel      one CTA per block of UB <= 128 users, streaming the whole catalogue in
+//                               tiles of 128 items:
+//            warp 8     TMA producer: item tiles [128 x 64] fp32, 128B-swizzled, 2-stage mbarrier ring
+//            warpgroups 0, 1  (64 users each): wgmma m64n128k8 kind tf32, 8 k-steps per tile, accumulators in
+//                       registers -> staged to shared memory row-major -> select: thread = one user row x one
+//                       64-column half of the tile, rated-item cursor, per-thread top-24 candidate list
+//                       (3 buckets of 8, minima in registers) in shared memory -> 2 x 24 candidates per user
 //          The raw fp32 tables are fed to the tensor core, which reads them as TF32 (low 13
 //          mantissa bits ignored): scores carry <= 2^-9 ||u|| ||i|| error -- candidates only.
 // Stage 3  tc_rescore_kernel    warp per user: exact fp32 fma-chain scores of the 2 x 24 candidates
@@ -32,26 +29,29 @@ namespace srb {
 using namespace tc;
 
 constexpr int TC_D = 64;          // embedding size handled by this kernel
-constexpr int TC_TN = 128;        // items per tile (UMMA N)
-constexpr int TC_STAGES = 2;      // smem ring depth (a tile's select takes ~2 us: one tile of prefetch is enough)
+constexpr int TC_TN = 128;        // items per tile (wgmma N)
+constexpr int TC_UB = 128;        // users per CTA: two consumer warpgroups of 64 (wgmma M)
+constexpr int TC_STAGES = 2;      // smem ring depth (a tile's select takes microseconds: one tile of prefetch is enough)
 constexpr int TC_LIST = 24;       // candidates per list; every user has two lists, one per column half of the tiles
 constexpr int TC_CAND = 2 * TC_LIST;
-constexpr int TC_EPI_WARPS = 16;
-constexpr int TC_THREADS = 64 + 32 * TC_EPI_WARPS;   // warp 0 TMA, warp 1 MMA, warps 2..17 epilogue
+constexpr int TC_THREADS = 256 + 32;   // warpgroups 0-1 MMA + select, warp 8 TMA
+constexpr int TC_SROW = TC_TN + 4;     // staged accumulator row stride (floats): conflict-free float4 row reads
 constexpr uint32_t TC_TILE_BYTES = TC_TN * TC_D * 4;     // 32 KB: 2 k-chunks x [128][32] fp32
-constexpr uint32_t TC_USER_BYTES = 2 * 128 * TC_D * 4;   // 64 KB: 2 halves x 2 k-chunks x [128][32]
+constexpr uint32_t TC_USER_BYTES = TC_UB * TC_D * 4;     // 32 KB: 2 k-chunks x [128][32]
 
 struct TcSmem {
   // dynamic shared memory, 1024-byte aligned base:
-  //   [0, 64K)          user tiles   half h, chunk c at (h*2 + c) * 16 KB
-  //   [64K, 64K+64K)    item stages  stage s, chunk c at 64K + s*32K + c*16K
-  //   then candidate lists: scores [24][512] f32, ids [24][512] i32   (96 KB)
+  //   [0, 32K)          user tile    chunk c at c * 16 KB (warpgroup w's 64 rows at + w * 8 KB)
+  //   [32K, 32K+64K)    item stages  stage s, chunk c at 32K + s*32K + c*16K
+  //   then the staged accumulators [2 warpgroups][64][TC_SROW] f32                  (66 KB)
+  //   then candidate lists: scores [24][256] f32, ids [24][256] i32               (48 KB)
   //   then barriers
   static constexpr uint32_t users_off = 0;
   static constexpr uint32_t items_off = TC_USER_BYTES;
-  static constexpr uint32_t cand_s_off = items_off + TC_STAGES * TC_TILE_BYTES;
-  static constexpr uint32_t cand_i_off = cand_s_off + TC_LIST * 512 * 4;
-  static constexpr uint32_t bar_off = cand_i_off + TC_LIST * 512 * 4;
+  static constexpr uint32_t stage_off = items_off + TC_STAGES * TC_TILE_BYTES;
+  static constexpr uint32_t cand_s_off = stage_off + TC_UB * TC_SROW * 4;
+  static constexpr uint32_t cand_i_off = cand_s_off + TC_LIST * 2 * TC_UB * 4;
+  static constexpr uint32_t bar_off = cand_i_off + TC_LIST * 2 * TC_UB * 4;
   static constexpr uint32_t total = bar_off + 256;
 };
 
@@ -61,7 +61,7 @@ struct TcArgs {
   const int32_t* rated_idx;
   int32_t n_q;
   int32_t n_items;
-  int32_t ub;                // users per CTA (<= 256)
+  int32_t ub;                // users per CTA (<= TC_UB)
   float* cand_s;             // [n_q][2][24] approx scores
   int32_t* cand_i;           // [n_q][2][24]
   int32_t* cand_n;           // [n_q][2]
@@ -96,11 +96,8 @@ tc_score_kernel(const __grid_constant__ CUtensorMap tm_users, const __grid_const
   uint8_t* sm = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(tc_smem_raw) + 1023) & ~(uintptr_t)1023);
   uint64_t* bars = reinterpret_cast<uint64_t*>(sm + TcSmem::bar_off);
   uint64_t* bar_full = bars;                    // [STAGES]  TMA -> MMA
-  uint64_t* bar_empty = bars + TC_STAGES;       // [STAGES]  MMA -> TMA
-  uint64_t* bar_tfull = bars + 2 * TC_STAGES;   // [2]       MMA -> epilogue
-  uint64_t* bar_tempty = bar_tfull + 2;         // [2]       epilogue -> MMA
-  uint64_t* bar_users = bar_tempty + 2;         // [1]
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bar_users + 1);
+  uint64_t* bar_empty = bars + TC_STAGES;       // [STAGES]  both warpgroups' MMAs done -> TMA
+  uint64_t* bar_users = bars + 2 * TC_STAGES;   // [1]
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
   const int q0 = blockIdx.x * a.ub;             // first query row of this CTA
@@ -109,33 +106,20 @@ tc_score_kernel(const __grid_constant__ CUtensorMap tm_users, const __grid_const
   if (threadIdx.x == 0) {
     for (int s = 0; s < TC_STAGES; ++s) {
       mbar_init(bar_full + s, 1);
-      mbar_init(bar_empty + s, 1);
-    }
-    for (int s = 0; s < 2; ++s) {
-      mbar_init(bar_tfull + s, 1);
-      mbar_init(bar_tempty + s, TC_EPI_WARPS);  // one arrive per epilogue warp
+      mbar_init(bar_empty + s, 2);  // one arrive per consumer warpgroup
     }
     mbar_init(bar_users, 1);
     fence_barrier_init();
   }
-  if (warp == 1) {
-    tmem_alloc(tmem_slot, 512);
-    tmem_relinquish();
-  }
-  fence_before_sync();
   __syncthreads();
-  fence_after_sync();
-  const uint32_t tmem = *tmem_slot;
 
-  if (warp == 0) {
+  if (warp == 8) {
     // ===== TMA producer =====
     if (elect_one()) {
       tma_prefetch_desc(&tm_users);
       tma_prefetch_desc(&tm_items);
       mbar_arrive_expect_tx(bar_users, TC_USER_BYTES);
-      for (int h = 0; h < 2; ++h)
-        for (int c = 0; c < 2; ++c)
-          tma_load_2d(sm + TcSmem::users_off + (h * 2 + c) * 16384, &tm_users, bar_users, c * 32, q0 + h * 128);
+      for (int c = 0; c < 2; ++c) tma_load_2d(sm + TcSmem::users_off + c * 16384, &tm_users, bar_users, c * 32, q0);
       for (int t = 0; t < n_tiles; ++t) {
         const int s = t % TC_STAGES;
         const uint32_t ph = (t / TC_STAGES) & 1;
@@ -145,164 +129,155 @@ tc_score_kernel(const __grid_constant__ CUtensorMap tm_users, const __grid_const
           tma_load_2d(sm + TcSmem::items_off + s * TC_TILE_BYTES + c * 16384, &tm_items, bar_full + s, c * 32, t * TC_TN);
       }
     }
-  } else if (warp == 1) {
-    // ===== MMA issuer =====
-    if (elect_one()) {
-      const uint32_t idesc = make_idesc_tf32(128, TC_TN);
-      mbar_wait(bar_users, 0);
-      for (int t = 0; t < n_tiles; ++t) {
-        const int s = t % TC_STAGES;
-        const int acc = t & 1;
-        mbar_wait(bar_tempty + acc, ((t >> 1) & 1) ^ 1);  // epilogue drained this accumulator stage
-        mbar_wait(bar_full + s, (t / TC_STAGES) & 1);
-        fence_after_sync();
-        const uint32_t items_base = smem_u32(sm + TcSmem::items_off + s * TC_TILE_BYTES);
+    return;
+  }
+  // ===== consumer warpgroup wg: MMA for its 64 users, then select: thread = one user row x one 64-column half =====
+  const int wg = warp >> 2;
+  const int lt = threadIdx.x & 127;
+  const int chalf = lt >> 6;      // column half of every tile
+  const int rloc = lt & 63;       // row within the warpgroup's 64
+  const int row = wg * 64 + rloc;
+  const int q = q0 + row;
+  const bool active = row < a.ub && q < a.n_q;
+  const int tix = chalf * TC_UB + row;  // column in the candidate arrays
+  float* cs = reinterpret_cast<float*>(sm + TcSmem::cand_s_off);
+  int32_t* ci = reinterpret_cast<int32_t*>(sm + TcSmem::cand_i_off);
+  float* stg = reinterpret_cast<float*>(sm + TcSmem::stage_off) + wg * 64 * TC_SROW;
+  constexpr int LS = 2 * TC_UB;  // candidate slot stride
+  float thr = -INFINITY;
+  int cnt = 0;
+  // cursor into this user's sorted rated list; the id after next is prefetched so that advancing the
+  // cursor never makes the warp wait for a global load
+  int cur = 0, cend = 0, next_rated = 0x7fffffff, after_next = 0x7fffffff;
+  if (active && a.rated_ptr) {
+    const int u = a.users[q];
+    cur = a.rated_ptr[u];
+    cend = a.rated_ptr[u + 1];
+    if (cur < cend) next_rated = a.rated_idx[cur];
+    if (cur + 1 < cend) after_next = a.rated_idx[cur + 1];
+  }
+  // candidate list: 24 (score, id) slots in shared memory (column `tix`), organised as 3 buckets of 8.
+  // Registers keep each bucket's minimum, so replacing the global minimum re-scans only one bucket
+  // (8 independent shared-memory loads) instead of the whole list.
+  // Each stored score carries its slot-in-bucket in the 3 low mantissa bits (the scores only rank candidates;
+  // the certificate in tc_rescore_kernel accounts for the 2^-20 relative perturbation), so a bucket's minimum
+  // names its own slot and 7 FMNMX replace a compare/select scan.
+  float bm0 = INFINITY, bm1 = INFINITY, bm2 = INFINITY;  // bucket minima (valid once full)
+  auto process_group = [&](const uint32_t (&r)[32], int g0) {
+    uint32_t mask = 0;
 #pragma unroll
-        for (int h = 0; h < 2; ++h) {
-          const uint32_t d_tmem = tmem + acc * 256 + h * 128;
-#pragma unroll
-          for (int c = 0; c < 2; ++c) {
-            const uint32_t ua = smem_u32(sm + TcSmem::users_off + (h * 2 + c) * 16384);
-            const uint32_t ib = items_base + c * 16384;
-#pragma unroll
-            for (int k = 0; k < 4; ++k)
-              umma_tf32_ss(d_tmem, make_smem_desc_k_sw128(ua + k * 32), make_smem_desc_k_sw128(ib + k * 32), idesc, (c | k) ? 1u : 0u);
-          }
-        }
-        umma_commit(bar_empty + s);     // smem stage reusable once these MMAs have read it
-        umma_commit(bar_tfull + acc);   // accumulators complete
-      }
+    for (int j = 0; j < 32; ++j)  // two instructions per score: FSETP + predicated LOP3
+      asm("{\n\t.reg .pred p;\n\tsetp.gt.f32 p, %1, %2;\n\t@p or.b32 %0, %0, %3;\n\t}"
+          : "+r"(mask)
+          : "f"(__uint_as_float(r[j])), "f"(thr), "r"(1u << j));
+    if (g0 + 32 > a.n_items) mask &= (g0 < a.n_items) ? (0xffffffffu >> (g0 + 32 - a.n_items)) : 0u;  // zero-filled OOB rows
+    if (!active) mask = 0;
+    // rated items never become candidates: walk the sorted rated list through this group
+    while (next_rated < g0 + 32) {
+      if (next_rated >= g0) mask &= ~(1u << (next_rated - g0));
+      ++cur;
+      next_rated = after_next;
+      after_next = (cur + 1 < cend) ? a.rated_idx[cur + 1] : 0x7fffffff;
     }
-  } else {
-    // ===== epilogue: 16 warps, thread = one user row x one 64-column half of every tile =====
-    const int e = warp - 2;
-    const int half = (e >> 2) & 1;  // user half (accumulator)
-    const int chalf = e >> 3;       // column half
-    const int quarter = warp & 3;   // TMEM lane quarter this warp may access
-    const int row = half * 128 + quarter * 32 + lane;
-    const int q = q0 + row;
-    const bool active = row < a.ub && q < a.n_q;
-    const int tix = chalf * 256 + row;  // column in the candidate arrays
-    float* cs = reinterpret_cast<float*>(sm + TcSmem::cand_s_off);
-    int32_t* ci = reinterpret_cast<int32_t*>(sm + TcSmem::cand_i_off);
-    float thr = -INFINITY;
-    int cnt = 0;
-    // cursor into this user's sorted rated list; the id after next is prefetched so that advancing the
-    // cursor never makes the warp wait for a global load
-    int cur = 0, cend = 0, next_rated = 0x7fffffff, after_next = 0x7fffffff;
-    if (active && a.rated_ptr) {
-      const int u = a.users[q];
-      cur = a.rated_ptr[u];
-      cend = a.rated_ptr[u + 1];
-      if (cur < cend) next_rated = a.rated_idx[cur];
-      if (cur + 1 < cend) after_next = a.rated_idx[cur + 1];
-    }
-    // candidate list: 24 (score, id) slots in shared memory (column `tix`), organised as 3 buckets of 8.
-    // Registers keep each bucket's minimum, so replacing the global minimum re-scans only one bucket
-    // (8 independent shared-memory loads) instead of the whole list.
-    // Each stored score carries its slot-in-bucket in the 3 low mantissa bits (the scores only rank candidates;
-    // the certificate in tc_rescore_kernel accounts for the 2^-20 relative perturbation), so a bucket's minimum
-    // names its own slot and 7 FMNMX replace a compare/select scan.
-    float bm0 = INFINITY, bm1 = INFINITY, bm2 = INFINITY;  // bucket minima (valid once full)
-    auto process_group = [&](const uint32_t (&r)[32], int g0) {
-      uint32_t mask = 0;
+    while (mask) {
+      const int j = __ffs(mask) - 1;
+      mask &= mask - 1;
+      // r[j] with a per-lane j: a 5-level select tree on the bits of j (31 selects)
+      uint32_t t16[16], t8[8], t4[4];
 #pragma unroll
-      for (int j = 0; j < 32; ++j)  // two instructions per score: FSETP + predicated LOP3
-        asm("{\n\t.reg .pred p;\n\tsetp.gt.f32 p, %1, %2;\n\t@p or.b32 %0, %0, %3;\n\t}"
-            : "+r"(mask)
-            : "f"(__uint_as_float(r[j])), "f"(thr), "r"(1u << j));
-      if (g0 + 32 > a.n_items) mask &= (g0 < a.n_items) ? (0xffffffffu >> (g0 + 32 - a.n_items)) : 0u;  // zero-filled OOB rows
-      if (!active) mask = 0;
-      // rated items never become candidates: walk the sorted rated list through this group
-      while (next_rated < g0 + 32) {
-        if (next_rated >= g0) mask &= ~(1u << (next_rated - g0));
-        ++cur;
-        next_rated = after_next;
-        after_next = (cur + 1 < cend) ? a.rated_idx[cur + 1] : 0x7fffffff;
-      }
-      while (mask) {
-        const int j = __ffs(mask) - 1;
-        mask &= mask - 1;
-        // r[j] with a per-lane j: a 5-level select tree on the bits of j (31 selects)
-        uint32_t t16[16], t8[8], t4[4];
+      for (int i = 0; i < 16; ++i) t16[i] = (j & 1) ? r[2 * i + 1] : r[2 * i];
 #pragma unroll
-        for (int i = 0; i < 16; ++i) t16[i] = (j & 1) ? r[2 * i + 1] : r[2 * i];
+      for (int i = 0; i < 8; ++i) t8[i] = (j & 2) ? t16[2 * i + 1] : t16[2 * i];
 #pragma unroll
-        for (int i = 0; i < 8; ++i) t8[i] = (j & 2) ? t16[2 * i + 1] : t16[2 * i];
+      for (int i = 0; i < 4; ++i) t4[i] = (j & 4) ? t8[2 * i + 1] : t8[2 * i];
+      const uint32_t t2a = (j & 8) ? t4[1] : t4[0], t2b = (j & 8) ? t4[3] : t4[2];
+      float sc = __uint_as_float((j & 16) ? t2b : t2a);
+      if (!(sc > thr)) continue;  // thr may have risen inside this group
+      const int id = g0 + j;
+      if (cnt < TC_LIST) {
+        cs[cnt * LS + tix] = sc;
+        ci[cnt * LS + tix] = id;
+        ++cnt;
+        if (cnt == TC_LIST) {  // list full: tag every slot and establish the bucket minima
 #pragma unroll
-        for (int i = 0; i < 4; ++i) t4[i] = (j & 4) ? t8[2 * i + 1] : t8[2 * i];
-        const uint32_t t2a = (j & 8) ? t4[1] : t4[0], t2b = (j & 8) ? t4[3] : t4[2];
-        float sc = __uint_as_float((j & 16) ? t2b : t2a);
-        if (!(sc > thr)) continue;  // thr may have risen inside this group
-        const int id = g0 + j;
-        if (cnt < TC_LIST) {
-          cs[cnt * 512 + tix] = sc;
-          ci[cnt * 512 + tix] = id;
-          ++cnt;
-          if (cnt == TC_LIST) {  // list full: tag every slot and establish the bucket minima
+          for (int b = 0; b < 3; ++b) {
+            float mn = INFINITY;
 #pragma unroll
-            for (int b = 0; b < 3; ++b) {
-              float mn = INFINITY;
-#pragma unroll
-              for (int qq = 0; qq < 8; ++qq) {
-                const float v = __uint_as_float((__float_as_uint(cs[(b * 8 + qq) * 512 + tix]) & ~7u) | (uint32_t)qq);
-                cs[(b * 8 + qq) * 512 + tix] = v;
-                mn = fminf(mn, v);
-              }
-              if (b == 0) bm0 = mn;
-              if (b == 1) bm1 = mn;
-              if (b == 2) bm2 = mn;
+            for (int qq = 0; qq < 8; ++qq) {
+              const float v = __uint_as_float((__float_as_uint(cs[(b * 8 + qq) * LS + tix]) & ~7u) | (uint32_t)qq);
+              cs[(b * 8 + qq) * LS + tix] = v;
+              mn = fminf(mn, v);
             }
-            thr = fminf(fminf(bm0, bm1), bm2);
+            if (b == 0) bm0 = mn;
+            if (b == 1) bm1 = mn;
+            if (b == 2) bm2 = mn;
           }
-        } else {
-          // evict the global minimum: it sits in the bucket whose minimum equals thr, in the slot its tag names
-          const int b = (bm0 == thr) ? 0 : ((bm1 == thr) ? 1 : 2);
-          const int pos = b * 8 + (int)(__float_as_uint(thr) & 7u);
-          cs[pos * 512 + tix] = __uint_as_float((__float_as_uint(sc) & ~7u) | (__float_as_uint(thr) & 7u));
-          ci[pos * 512 + tix] = id;
-          float mn = cs[(b * 8) * 512 + tix];
-#pragma unroll
-          for (int qq = 1; qq < 8; ++qq) mn = fminf(mn, cs[(b * 8 + qq) * 512 + tix]);
-          if (b == 0) bm0 = mn;
-          else if (b == 1) bm1 = mn;
-          else bm2 = mn;
           thr = fminf(fminf(bm0, bm1), bm2);
         }
+      } else {
+        // evict the global minimum: it sits in the bucket whose minimum equals thr, in the slot its tag names
+        const int b = (bm0 == thr) ? 0 : ((bm1 == thr) ? 1 : 2);
+        const int pos = b * 8 + (int)(__float_as_uint(thr) & 7u);
+        cs[pos * LS + tix] = __uint_as_float((__float_as_uint(sc) & ~7u) | (__float_as_uint(thr) & 7u));
+        ci[pos * LS + tix] = id;
+        float mn = cs[(b * 8) * LS + tix];
+#pragma unroll
+        for (int qq = 1; qq < 8; ++qq) mn = fminf(mn, cs[(b * 8 + qq) * LS + tix]);
+        if (b == 0) bm0 = mn;
+        else if (b == 1) bm1 = mn;
+        else bm2 = mn;
+        thr = fminf(fminf(bm0, bm1), bm2);
       }
-    };
-    for (int t = 0; t < n_tiles; ++t) {
-      const int acc = t & 1;
-      mbar_wait(bar_tfull + acc, (t >> 1) & 1);
-      fence_after_sync();
-      const int n0 = t * TC_TN;
-      const uint32_t tbase = tmem + ((uint32_t)(quarter * 32) << 16) + acc * 256 + half * 128 + chalf * 64;
-      const int c0 = n0 + chalf * 64;
-      // two register buffers: the load of the second group is in flight while the first is processed
-      uint32_t r0[32], r1[32];
-      tmem_ld_32x32(tbase, r0);
-      tmem_ld_wait();
-      tmem_ld_32x32(tbase + 32, r1);
-      process_group(r0, c0);
-      tmem_ld_wait();
-      fence_before_sync();  // my share of the accumulator is in registers: hand the stage back before selecting
-      __syncwarp();
-      if (lane == 0) mbar_arrive(bar_tempty + acc);
-      process_group(r1, c0 + 32);
     }
-    if (active) {
-      const size_t o = ((size_t)q * 2 + chalf) * TC_LIST;
-      for (int p = 0; p < TC_LIST; ++p) {
-        a.cand_s[o + p] = (p < cnt) ? cs[p * 512 + tix] : -INFINITY;
-        a.cand_i[o + p] = (p < cnt) ? ci[p * 512 + tix] : -1;
+  };
+  const uint32_t ua = smem_u32(sm + TcSmem::users_off + wg * 8192);
+  const int w4 = warp & 3, g = lane >> 2, tq = lane & 3;
+  mbar_wait(bar_users, 0);
+  for (int t = 0; t < n_tiles; ++t) {
+    const int s = t % TC_STAGES;
+    mbar_wait(bar_full + s, (t / TC_STAGES) & 1);
+    float acc[64];
+    const uint32_t ib = smem_u32(sm + TcSmem::items_off + s * TC_TILE_BYTES);
+    wgmma_fence();
+#pragma unroll
+    for (int c = 0; c < 2; ++c)
+#pragma unroll
+      for (int k = 0; k < 4; ++k)
+        wgmma_m64n128k8_tf32_ss(acc, make_smem_desc_k_sw128(ua + c * 16384 + k * 32), make_smem_desc_k_sw128(ib + c * 16384 + k * 32),
+                                (c | k) ? 1u : 0u);
+    wgmma_commit();
+    wgmma_wait<0>();
+    if (lt == 0) mbar_arrive(bar_empty + s);  // this warpgroup is done reading the stage
+    named_bar_sync(1 + wg, 128);             // the previous tile's staged scores have been read
+#pragma unroll
+    for (int j = 0; j < 64; j += 2) {
+      const int rr = w4 * 16 + g + 8 * ((j >> 1) & 1);
+      const int cc = 8 * (j >> 2) + 2 * tq;
+      *reinterpret_cast<float2*>(stg + rr * TC_SROW + cc) = make_float2(acc[j], acc[j + 1]);
+    }
+    named_bar_sync(1 + wg, 128);
+    const int c0 = t * TC_TN + chalf * 64;
+    const float* src = stg + rloc * TC_SROW + chalf * 64;
+    uint32_t r[32];
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+#pragma unroll
+      for (int j = 0; j < 32; j += 4) {
+        const float4 v = *reinterpret_cast<const float4*>(src + h * 32 + j);
+        r[j] = __float_as_uint(v.x), r[j + 1] = __float_as_uint(v.y), r[j + 2] = __float_as_uint(v.z), r[j + 3] = __float_as_uint(v.w);
       }
-      a.cand_n[(size_t)q * 2 + chalf] = cnt;
-      a.cand_thr[(size_t)q * 2 + chalf] = (cnt == TC_LIST) ? thr : -INFINITY;
+      process_group(r, c0 + h * 32);
     }
   }
-  fence_before_sync();
-  __syncthreads();
-  if (warp == 1) tmem_dealloc(tmem, 512);
+  if (active) {
+    const size_t o = ((size_t)q * 2 + chalf) * TC_LIST;
+    for (int p = 0; p < TC_LIST; ++p) {
+      a.cand_s[o + p] = (p < cnt) ? cs[p * LS + tix] : -INFINITY;
+      a.cand_i[o + p] = (p < cnt) ? ci[p * LS + tix] : -1;
+    }
+    a.cand_n[(size_t)q * 2 + chalf] = cnt;
+    a.cand_thr[(size_t)q * 2 + chalf] = (cnt == TC_LIST) ? thr : -INFINITY;
+  }
 }
 
 struct RescoreArgs {
@@ -517,7 +492,7 @@ int score_topk_fallback(const srb_topk_desc* d, const int32_t* fb_users, const i
                         float* scratch, int fb_cap, cudaStream_t st);  // score_topk.cu
 
 int score_topk_tc(const srb_topk_desc* d, cudaStream_t st) {
-  SRB_REQUIRE(d->d == TC_D, "topk impl 2 (tcgen05) supports d=64 only (got %d)", d->d);
+  SRB_REQUIRE(d->d == TC_D, "topk impl 2 (tensor cores) supports d=64 only (got %d)", d->d);
   const int n_q = d->n_q;
   const TcWorkspace need = tc_carve(nullptr, n_q, d->n_items);
   SRB_REQUIRE(d->workspace && d->workspace_bytes >= need.bytes, "topk impl 2: workspace too small (%lld < %lld)",
@@ -534,15 +509,16 @@ int score_topk_tc(const srb_topk_desc* d, cudaStream_t st) {
                                                                 d->n_items, w.bmax);
     SRB_TRY(post_launch("tc_gather_kernel"));
   }
-  // users per CTA: spread the queries over one wave of SMs, multiple of 32, at most 256
+  // users per CTA: one wave of SMs when the queries fit (n_q <= TC_UB x SMs), else TC_UB per CTA and several waves
+  // (yelp2018: 31 668 users -> 248 CTAs on 132 SMs, one CTA per SM at ~211 KB of shared memory); multiple of 32
   const int sms = sm_count();
   int ub = (n_q + sms - 1) / sms;
   ub = (ub + 31) / 32 * 32;
-  if (ub > 256) ub = 256;
+  if (ub > TC_UB) ub = TC_UB;
   if (ub < 32) ub = 32;
   const int blocks = (n_q + ub - 1) / ub;
   CUtensorMap tm_users, tm_items;
-  SRB_REQUIRE(make_tmap_f32_rows(&tm_users, w.ug, (uint64_t)n_q_pad, TC_D, 128) == 0, "topk impl 2: cuTensorMapEncodeTiled(users) failed");
+  SRB_REQUIRE(make_tmap_f32_rows(&tm_users, w.ug, (uint64_t)n_q_pad, TC_D, TC_UB) == 0, "topk impl 2: cuTensorMapEncodeTiled(users) failed");
   SRB_REQUIRE(make_tmap_f32_rows(&tm_items, d->item_emb, (uint64_t)d->n_items, TC_D, TC_TN) == 0,
               "topk impl 2: cuTensorMapEncodeTiled(items) failed");
   TcArgs a;

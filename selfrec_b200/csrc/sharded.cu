@@ -4,8 +4,8 @@
 // u % world == g (local row u / world): their rows of every [U, d] table (parameters, moments, layer buffers) never
 // leave the GPU.  The cyclic assignment gives every rank the same mix of heavy and light users -- ids follow first
 // appearance in the training file (ui_graph.py:29-40), so on a power-law graph contiguous nnz-balanced blocks put a
-// few hundred hub users on rank 0 and millions of cold ones on the last rank, whose products then take 1.5x longer
-// (profiles/r02l_trace_10M_n2_barrier.txt).  The (5-50x smaller) ITEM tables are replicated.  One propagation layer is
+// few hundred hub users on rank 0 and millions of cold ones on the last rank, whose products (cold gathers, far more
+// rows to write) then take much longer.  The (5-50x smaller) ITEM tables are replicated.  One propagation layer is
 //     X_u' [block g] = R_g  X_i                 local SpMM over the replicated item table, nothing to exchange
 //     X_i'           = sum_g R_g^T X_u[block g]  every rank contributes a partial [I, d] product
 // and only the item half crosses NVLink: the item-side SpMM stores each finished partial row straight into the
@@ -299,9 +299,8 @@ static bool sync_in_kernels() {
 
 // NVLS route of the partial-sum exchange (needs the multicast mapping): partial products stay in the rank's own copy of
 // the staging buffer and the owner reads their sum with multimem.ld_reduce.  Opt-in (srb_shard_desc.nvls; parity-tested
-// like the default): at 2 ranks the in-switch reduction delivered 183 GB/s per GPU and the step took 91 ms against 82 ms
-// with the P2P pushes (profiles/r02o_trace_10M_n2_*.txt) -- it halves a rank's NVLink ingress, which only matters from
-// 4-8 ranks.
+// like the default): it halves a rank's NVLink ingress, which only matters from 4-8 ranks, at the price of an in-switch
+// reduction whose rate bounds the owner's read.
 static bool nvls(const Ctx& c) { return c.s->nvls != 0 && c.G > 1 && c.s->sym_mc != nullptr; }
 
 // wait / signal folded into the kernels of a layer (PeerSync in spmm_args.cuh)

@@ -135,8 +135,8 @@ __device__ __forceinline__ void spmm_epilogue(const SpmmArgs& a, int row, int gl
 
 // Mapping: a row vector of D floats lives on LPR = D/8 lanes (two float4 per lane: columns
 // [4*gl, 4*gl+4) and [D/2 + 4*gl, ...)).  Rows are taken in `row_order` (degree-descending), in three
-// classes so that no row is a long chain of dependent L2 round trips (~1.7 us each under load; a
-// 1600-non-zero row handled by one warp alone took as long as the rest of the matrix):
+// classes so that no row is a long chain of dependent L2 round trips (a row of thousands of non-zeros handled by
+// one warp alone would take as long as the rest of the matrix):
 //   * the first n_vlong rows get a whole CTA: 8 warps x 4 lane groups stride through the row, partial
 //     sums meet in shared memory;
 //   * the next n_long rows get a warp each (the 32/LPR lane groups stride 32 non-zeros per iteration
@@ -681,8 +681,8 @@ int launch_spmm(const SpmmArgs& a, int d, cudaStream_t st) {
 }
 
 // SRB_SPMM_ASYNC=1 stages every second gather sub-batch through cp.async + shared memory (measurement switch; results
-// are bit-identical).  Off by default: at config-5 size it measured 22.4 ms per product against 19.6 ms on the register
-// path (profiles/r02l_probe10M_*.json) -- twice the bytes in flight did not help, the LDGSTS + LDS round trip cost more.
+// are bit-identical).  Off by default: it doubles the bytes in flight, but every staged row pays an LDGSTS + LDS round
+// trip through the shared-memory port; run tools/config5_probe.py with and without it to compare.
 static bool async_stage_enabled() {
   static const int on = [] {
     const char* e = getenv("SRB_SPMM_ASYNC");
@@ -754,9 +754,9 @@ int fill_args(const srb_spmm_desc* d, SpmmArgs& a) {
   a.noise_row_stride = 1;
   a.peer_mc = 0;
   a.ps = PeerSync{};
-  // (rows + columns) x d x 4 bytes of dense operands beyond ~3/4 of the 126 MB L2: stream the one-touch data
-  a.stream = ((long long)d->n_rows + d->n_cols) * d->d * 4 > (96ll << 20);
-  a.async_stage = a.stream && async_stage_enabled();  // (opt-in: measured slower, profiles/README.md r02l)
+  // (rows + columns) x d x 4 bytes of dense operands beyond 3/4 of the L2 (37.5 MB on an H100): stream the one-touch data
+  a.stream = ((long long)d->n_rows + d->n_cols) * d->d * 4 > l2_bytes() / 4 * 3;
+  a.async_stage = a.stream && async_stage_enabled();  // (opt-in measurement switch, see async_stage_enabled)
   a.stage_rank = a.stage_cap = 0;
   for (int g = 0; g < 8; ++g) a.peer[g] = a.peer_sum[g] = a.peer_p[g] = a.stage_peer[g] = nullptr;
   for (int g = 0; g < 9; ++g) a.stage_bounds[g] = 0;

@@ -1,7 +1,7 @@
 """Torch-facing wrappers over the C ABI (selfrec_b200/_lib.py).
 
 PyTorch is plumbing here: it owns device memory, streams and autograd bookkeeping; every
-computation is a hand-written sm_100a kernel reached through ctypes with raw pointers.
+computation is a hand-written sm_90a kernel reached through ctypes with raw pointers.
 All ops are stream-ordered on torch's current stream and raise SrbError without a GPU.
 """
 import ctypes as C
@@ -70,16 +70,29 @@ def classify_rows(rowptr):
     return out
 
 
-HUB_BLOCK_BYTES = 32 << 20  # X rows of one column block of the column-blocked split-row lists
+HUB_BLOCK_BYTES = None  # X rows of one column block of the column-blocked split-row lists; None: a quarter of the L2
+
+
+def hub_block_bytes(device):
+    """Column-block size of the split-row lists: a quarter of the device's L2 (12.5 MB on an H100), so that one block
+    of X stays resident next to the CSR and output streams.  HUB_BLOCK_BYTES overrides it."""
+    if HUB_BLOCK_BYTES is not None:
+        return HUB_BLOCK_BYTES
+    device = torch.device(device)
+    if device.type != "cuda":  # lists built from host tensors: the current GPU's L2, else the H100's 50 MB
+        if not torch.cuda.is_available():
+            return (50 << 20) // 4
+        device = torch.device("cuda", torch.cuda.current_device())
+    return torch.cuda.get_device_properties(device).L2_cache_size // 4
 
 
 def column_blocked_segments(rowptr, colidx, rows, n_cols, d):
     """Column-blocked work lists of the split rows `rows` (device tensors; srb_hub_split.seg in the header): every
-    split row is cut at column-block boundaries (block = HUB_BLOCK_BYTES of X rows) and at most HUB_CHUNK non-zeros,
+    split row is cut at column-block boundaries (block = hub_block_bytes() of X rows) and at most HUB_CHUNK non-zeros,
     and the segments are ordered by (column block, row) so that one block of X stays L2-resident while ALL rows'
     segments of that block are processed.  Returns dict(seg, first, cnt, order_cta, order_warp) or None when the
     matrix has a single column block."""
-    W = max(4096, HUB_BLOCK_BYTES // (4 * d))
+    W = max(4096, hub_block_bytes(rowptr.device) // (4 * d))
     if n_cols <= 2 * W or rows.numel() == 0:
         return None
     dev = rowptr.device

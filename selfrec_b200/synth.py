@@ -111,7 +111,8 @@ def make_interaction(shape="yelp2018", seed=0, scale=1.0):
 # ------------------------------------------------------------------------------------------------
 # config-5 sized graphs: generated, relabelled and normalised on the GPU (no scipy / no Python lists at 200 M edges)
 # ------------------------------------------------------------------------------------------------
-SHAPES["synthetic-10M"] = (10_000_000, 2_000_000, 200_000_000)   # BASELINE.json configs[4]
+SHAPES["synthetic-10M"] = (10_000_000, 2_000_000, 200_000_000)   # BASELINE.json configs[4] (about 100 GB of device memory at d = 128)
+SHAPES["synthetic-5M"] = (5_000_000, 1_000_000, 100_000_000)     # the same recipe at half the rows: fits one 80 GB GPU
 SHAPES["synthetic-2M"] = (2_000_000, 500_000, 40_000_000)        # mid-size stand-in (same recipe, 1/5 of the rows)
 
 

@@ -394,6 +394,60 @@ def test_op_level_dropin_runs_reference_style_train_body(torch_cuda, golden, tin
         np.testing.assert_allclose(got, fx[f"params_after_{k}"], rtol=RTOL, atol=1e-6)
 
 
+@pytest.mark.parametrize("name", ["XSimGCL", "SimGCL"])
+def test_op_level_dropin_contrastive_train_body(torch_cuda, golden, tiny, name):
+    """The reference's XSimGCL / SimGCL train() bodies (XSimGCL.py:27-37, 83-101 and :46-50; SimGCL.py:25-36, 81-93 and
+    :43-50) written against the drop-in modules only -- torch.sparse.mm(handle, E), the perturbed encoder with the
+    recorded rand_like draws, bpr_loss, l2_reg_loss, InfoNCE over the unique batch ids, torch.optim.Adam -- must
+    reproduce the reference's parameters step for step."""
+    torch = torch_cuda
+    import torch.nn.functional as F
+    from selfrec_b200.base.torch_interface import TorchGraphInterface
+    from selfrec_b200.util.loss_torch import InfoNCE, bpr_loss, l2_reg_loss
+    fx = golden(f"train_{name}.npz")
+    U = tiny["U"]
+    n_layers, eps, cl_rate, tau = (3, 0.2, 0.2, 0.2) if name == "XSimGCL" else (2, 0.1, 0.5, 0.2)
+    ue = torch.nn.Parameter(torch.from_numpy(fx["init_user"]).cuda())
+    ie = torch.nn.Parameter(torch.from_numpy(fx["init_item"]).cuda())
+    A = TorchGraphInterface.convert_sparse_mat_to_tensor(tiny["norm"]).cuda()
+    opt = torch.optim.Adam([ue, ie], lr=0.001)
+    draws = iter(fx["noise"])  # the reference's torch.rand_like draws, in call order
+
+    def encoder(perturbed):
+        ego = torch.cat([ue, ie], 0)
+        layers, cl = [], ego
+        for k in range(n_layers):
+            ego = torch.sparse.mm(A, ego)
+            if perturbed:
+                noise = torch.from_numpy(next(draws)).cuda()
+                ego = ego + torch.sign(ego) * F.normalize(noise, dim=-1) * eps
+            layers.append(ego)
+            if k == 0:  # XSimGCL's l* = 1
+                cl = ego
+        out = torch.mean(torch.stack(layers, dim=1), dim=1)
+        return out[:U], out[U:], cl[:U], cl[U:]
+
+    for k in range(int(fx["n_steps"])):
+        u, i, j = (fx[f"b{k}_{t}"].tolist() for t in ("u", "i", "j"))
+        u_idx = torch.unique(torch.tensor(u, dtype=torch.long)).cuda()
+        i_idx = torch.unique(torch.tensor(i, dtype=torch.long)).cuda()
+        if name == "XSimGCL":
+            ru, ri, cu, ci = encoder(True)
+            cl_loss = InfoNCE(ru[u_idx], cu[u_idx], tau) + InfoNCE(ri[i_idx], ci[i_idx], tau)
+        else:
+            ru, ri, _, _ = encoder(False)
+            v1u, v1i, _, _ = encoder(True)
+            v2u, v2i, _, _ = encoder(True)
+            cl_loss = InfoNCE(v1u[u_idx], v2u[u_idx], tau) + InfoNCE(v1i[i_idx], v2i[i_idx], tau)
+        loss = bpr_loss(ru[u], ri[i], ri[j]) + l2_reg_loss(0.0001, ru[u], ri[i]) + cl_rate * cl_loss
+        opt.zero_grad()
+        loss.backward()
+        opt.step()
+        got = torch.cat([ue, ie]).detach().cpu().numpy()
+        np.testing.assert_allclose(got, fx[f"params_after_{k}"], rtol=RTOL, atol=1e-6, err_msg=f"{name} step {k}")
+    assert next(draws, None) is None, "every recorded noise draw is consumed"
+
+
 # ------------------------------------------------------------------------------------------
 # (iv) scoring + top-k
 # ------------------------------------------------------------------------------------------

@@ -1,4 +1,4 @@
-"""Tensor-core scoring (impl 2: tcgen05 TF32 candidates + exact fp32 re-scoring) must return
+"""Tensor-core scoring (impl 2: wgmma TF32 candidates + exact fp32 re-scoring) must return
 exactly what the CUDA-core kernel (impl 1, bit-identical to the oracle) returns."""
 import numpy as np
 import pytest

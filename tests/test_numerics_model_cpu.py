@@ -2,7 +2,7 @@
 
 * 3xTF32 (csrc/infonce_tc.cuh): x = hi + lo with hi = rna_tf32(x), lo truncated to TF32; hi*hi + hi*lo + lo*hi
   reproduces an fp32 dot product to ~2^-21 relative, a single TF32 pass only to ~2^-11.
-* the exactness certificate of the tcgen05 ranking path (csrc/score_topk_tc.cu): with TF32-truncated operands
+* the exactness certificate of the tensor-core ranking path (csrc/score_topk_tc.cu): with TF32-truncated operands
   every approximate score is within E = (2^-9 + 2^-16 + 2^-18) * ||u|| * max||i|| of the exact one, so if the best
   non-candidate bound max(thr_A, thr_B) + E is below the exact k-th score, the true top-k lies inside the
   2 x 24 candidates -- whatever the data; and the pruning rule of tc_rescore_kernel (drop candidates whose approximate

@@ -7,7 +7,7 @@ de-duplicated, first-appearance ids; here the 1/5-size shape synthetic-2M so tha
   * how contiguous nnz-balanced user blocks compare with the cyclic assignment (rows per rank), and how many
     (rank, item) partial rows of the item-side product are empty.
 
-    python tools/hotset_sim.py [shape] > profiles/r02q_hotset_sim_2M.txt
+    python tools/hotset_sim.py [shape]
 """
 import os
 import sys

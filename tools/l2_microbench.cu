@@ -1,5 +1,5 @@
 // L2 / HBM gather-bandwidth microbenchmark (evidence for DESIGN.md: the SpMM's X-row gathers
-// are bound by L2->SM throughput).  nvcc -gencode arch=compute_100a,code=sm_100a -O3 -o l2mb l2_microbench.cu
+// are bound by L2->SM throughput).  nvcc -gencode arch=compute_90a,code=sm_90a -O3 -o l2mb l2_microbench.cu
 #include <cuda_runtime.h>
 #include <stdio.h>
 #include <stdlib.h>

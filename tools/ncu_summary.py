@@ -1,4 +1,4 @@
-"""Summarise an .ncu-rep (read here on the CPU box with `ncu -i`) into a small CSV for profiles/."""
+"""Summarise an .ncu-rep (read with `ncu -i`, no GPU needed) into a small CSV of the metrics below."""
 import csv, subprocess, sys
 KEEP = ["gpu__time_duration.sum", "dram__bytes_read.sum", "dram__bytes_write.sum", "lts__t_sector_hit_rate.pct",
         "l1tex__t_sector_hit_rate.pct", "lts__throughput.avg.pct_of_peak_sustained_elapsed", "l1tex__throughput.avg.pct_of_peak_sustained_elapsed",

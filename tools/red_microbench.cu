@@ -1,6 +1,6 @@
 // How fast can the L2 absorb red.global.add.v4.f32 row updates (256 B rows, random rows of a 17.8 MB
 // table)?  Decides whether the row-sparse backward product should push (scatter) instead of pull.
-// nvcc -gencode arch=compute_100a,code=sm_100a -O3 -o red_mb red_microbench.cu
+// nvcc -gencode arch=compute_90a,code=sm_90a -O3 -o red_mb red_microbench.cu
 #include <cstdio>
 #include <cstdint>
 #include <cuda_runtime.h>
@@ -38,8 +38,10 @@ int main() {
   cudaEvent_t e0, e1;
   cudaEventCreate(&e0);
   cudaEventCreate(&e1);
+  int sms = 0;
+  cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, 0);
   for (int upd : {8, 32, 128}) {
-    for (int blocks : {148 * 2, 148 * 8}) {
+    for (int blocks : {sms * 2, sms * 8}) {
       const long long groups = (long long)blocks * 256 / 8;
       for (int kind = 0; kind < 2; ++kind) {
         for (int w = 0; w < 2; ++w) (kind ? store_rows : push_rows)<<<blocks, 256>>>(Y, n_rows, upd, 7u);

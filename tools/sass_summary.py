@@ -1,7 +1,9 @@
 #!/usr/bin/env python
 """Per-kernel SASS mnemonic counts of libselfrec_b200.so (cuobjdump -sass): the evidence that the tensor-core
-kernels really are tcgen05 + TMEM + TMA (UTCHMMA / UTCBAR / LDTM / STTM / UTMALDG, B200_PROFILING.md) and that the
-HBM-bound ones use 128-bit accesses.  Writes profiles/r02_sass_summary.txt."""
+kernels really are wgmma + TMA (HGMMA / WARPGROUP / UTMALDG / SYNCS) and that the HBM-bound ones use 128-bit accesses.
+
+    python tools/sass_summary.py [out.txt]          (default: stdout)
+"""
 import collections
 import os
 import re
@@ -10,7 +12,7 @@ import sys
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 LIB = os.path.join(ROOT, "selfrec_b200", "libselfrec_b200.so")
-WATCH = ["UTCHMMA", "UTCQMMA", "UTCBAR", "UTMALDG", "UBLKCP", "LDTM", "STTM", "UTCATOMSWS", "SYNCS", "LDG.E.128", "LDG.E.64", "STG.E.128", "RED.E",
+WATCH = ["HGMMA", "WARPGROUP", "UTMALDG", "UBLKCP", "SYNCS", "LDG.E.128", "LDG.E.64", "STG.E.128", "RED.E",
          "REDG", "ATOMG", "LDS.128", "FFMA", "FMNMX3", "FMNMX", "SHFL", "MUFU.EX2", "BAR.SYNC", "CCTL"]
 
 
@@ -34,17 +36,19 @@ def main():
             for w in WATCH:
                 if op == w or op.startswith(w + ".") or (w.count(".") and op.startswith(w)):
                     cur[w] += 1
-    lines = ["# SASS mnemonic counts per kernel: cuobjdump -sass selfrec_b200/libselfrec_b200.so (sm_100a), round 2",
+    lines = ["# SASS mnemonic counts per kernel: cuobjdump -sass selfrec_b200/libselfrec_b200.so (sm_90a)",
              "# columns: instructions | " + " ".join(WATCH), ""]
     for name, c in kernels.items():
         hits = " ".join(f"{w}={c[w]}" for w in WATCH if c[w])
         lines.append(f"{name:<60s} {c['_total']:6d} | {hits}")
-    tc = [n for n, c in kernels.items() if c["UTCHMMA"]]
-    lines += ["", f"kernels issuing tcgen05.mma (UTCHMMA): {len(tc)}: " + ", ".join(tc)]
-    path = os.path.join(ROOT, "profiles", "r02_sass_summary.txt")
-    with open(path, "w") as f:
-        f.write("\n".join(lines) + "\n")
-    print(path, len(kernels), "kernels;", len(tc), "with UTCHMMA")
+    tc = [n for n, c in kernels.items() if c["HGMMA"]]
+    lines += ["", f"kernels issuing wgmma (HGMMA): {len(tc)}: " + ", ".join(tc)]
+    text = "\n".join(lines) + "\n"
+    if len(sys.argv) > 1:
+        with open(sys.argv[1], "w") as f:
+            f.write(text)
+    else:
+        sys.stdout.write(text)
 
 
 if __name__ == "__main__":
