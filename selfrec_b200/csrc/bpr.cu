@@ -46,6 +46,8 @@ __global__ void __launch_bounds__(256) bpr_reduce_kernel(const BprArgs a) {
   const int lane = threadIdx.x & 31;
   const int wib = threadIdx.x >> 5;
   const int t = blockIdx.x * (blockDim.x >> 5) + wib;
+  pdl_wait();
+  pdl_trigger();
   const int b = a.b_dev ? min(*a.b_dev, a.b) : a.b;
   float bpr = 0.f, su = 0.f, sp = 0.f, sn = 0.f;
   if (t < b) {
@@ -100,6 +102,8 @@ __global__ void __launch_bounds__(256) bpr_grad_kernel(const BprArgs a) {
   constexpr int Q = (D + 127) / 128;
   const int lane = threadIdx.x & 31;
   const int t = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
+  pdl_wait();
+  pdl_trigger();
   const int b = a.b_dev ? min(*a.b_dev, a.b) : a.b;
   const float fb = (float)b;
   const float nu = sqrtf(a.scratch[1]), np = sqrtf(a.scratch[2]), nn = sqrtf(a.scratch[3]);
@@ -171,6 +175,8 @@ __global__ void __launch_bounds__(256) scatter_add_rows_kernel(float* dst, const
   const ScatterSeg& sg = segs.s[blockIdx.y];
   const int lane = threadIdx.x & 31;
   const int r = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
+  pdl_wait();
+  pdl_trigger();
   const int nn = sg.n_dev ? min(*sg.n_dev, sg.n) : sg.n;
   if (r >= nn) return;
   int row = sg.rows[r] + sg.row_off;
@@ -194,12 +200,11 @@ int scatter_segments(float* dst, int d, const ScatterSegs& segs, cudaStream_t st
   if (max_n == 0) return SRB_OK;
   dim3 grid((max_n + 7) / 8, segs.count);
   switch (d) {
-    case 32: scatter_add_rows_kernel<32><<<grid, 256, 0, st>>>(dst, segs); break;
-    case 64: scatter_add_rows_kernel<64><<<grid, 256, 0, st>>>(dst, segs); break;
-    case 128: scatter_add_rows_kernel<128><<<grid, 256, 0, st>>>(dst, segs); break;
+    case 32: return launch_kernel(scatter_add_rows_kernel<32>, grid, 256, 0, st, "scatter_add_rows_kernel", dst, segs);
+    case 64: return launch_kernel(scatter_add_rows_kernel<64>, grid, 256, 0, st, "scatter_add_rows_kernel", dst, segs);
+    case 128: return launch_kernel(scatter_add_rows_kernel<128>, grid, 256, 0, st, "scatter_add_rows_kernel", dst, segs);
     default: set_error("scatter: unsupported d=%d (32, 64, 128)", d); return SRB_ERR_ARG;
   }
-  return post_launch("scatter_add_rows_kernel");
 }
 
 // Standalone l2_reg_loss (util/loss_torch.py:18-22) for the op-level drop-in, where the
@@ -248,17 +253,14 @@ __global__ void __launch_bounds__(256) l2_grad_kernel(const L2Args a, const floa
 }
 
 __global__ void adam_prepare_kernel(int32_t* step, float* scalars, double lr, double b1, double b2) {
-  const int t = *step + 1;
-  *step = t;
-  const double bc1 = 1.0 - pow(b1, (double)t);
-  const double bc2 = 1.0 - pow(b2, (double)t);
-  scalars[0] = (float)(lr / bc1);
-  scalars[1] = (float)sqrt(bc2);
+  adam_prepare(step, scalars, lr, b1, b2);
 }
 
 __global__ void __launch_bounds__(256) adam_step_kernel(float* __restrict__ p, float* __restrict__ m, float* __restrict__ v,
                                                         const float* __restrict__ g, long long n4, long long n,
                                                         const float* __restrict__ scal, float w1, float b2, float w2, float eps) {
+  pdl_wait();
+  pdl_trigger();
   const float step_size = scal[0], bc2_sqrt = scal[1];
   const long long stride = (long long)gridDim.x * blockDim.x;
   for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n4; i += stride) {
@@ -319,12 +321,10 @@ extern "C" int srb_bpr_l2_fwd_bwd(const srb_bpr_desc* d, void* stream) {
   SRB_TRY(srb::check_cuda(cudaMemsetAsync(d->scratch, 0, 8 * sizeof(float), st), "bpr memset"));
   const int blocks = d->b > 0 ? (d->b + 7) / 8 : 1;
   switch (d->d) {
-#define SRB_CASE(DD)                                               \
-  case DD:                                                         \
-    srb::bpr_reduce_kernel<DD><<<blocks, 256, 0, st>>>(a);         \
-    SRB_TRY(srb::post_launch("bpr_reduce_kernel"));                \
-    srb::bpr_grad_kernel<DD><<<blocks, 256, 0, st>>>(a);           \
-    return srb::post_launch("bpr_grad_kernel");
+#define SRB_CASE(DD)                                                                                 \
+  case DD:                                                                                           \
+    SRB_TRY(srb::launch_kernel(srb::bpr_reduce_kernel<DD>, blocks, 256, 0, st, "bpr_reduce_kernel", a)); \
+    return srb::launch_kernel(srb::bpr_grad_kernel<DD>, blocks, 256, 0, st, "bpr_grad_kernel", a);
     SRB_CASE(32)
     SRB_CASE(64)
     SRB_CASE(128)
@@ -371,9 +371,8 @@ extern "C" int srb_adam_step(float* p, float* m, float* v, const float* g, int64
   const long long cap = (long long)srb::sm_count() * 8;
   if (blocks > cap) blocks = cap;
   if (blocks < 1) blocks = 1;
-  srb::adam_step_kernel<<<(int)blocks, 256, 0, (cudaStream_t)stream>>>(p, m, v, g, n4, n, scalars_dev, (float)(1.0 - beta1), (float)beta2,
-                                                                        (float)(1.0 - beta2), eps);
-  return srb::post_launch("adam_step_kernel");
+  return srb::launch_kernel(srb::adam_step_kernel, (int)blocks, 256, 0, (cudaStream_t)stream, "adam_step_kernel", p, m, v, g, n4, n,
+                            scalars_dev, (float)(1.0 - beta1), (float)beta2, (float)(1.0 - beta2), eps);
 }
 
 extern "C" int srb_l2_reg_fwd(int32_t n_terms, const float* const* x, const int64_t* n_elems, const int32_t* rows, float reg,

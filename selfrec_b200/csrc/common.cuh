@@ -4,6 +4,7 @@
 #include <stdint.h>
 #include <stdio.h>
 #include <atomic>
+#include <utility>
 #include "selfrec_b200.h"
 
 #define SRB_FULL_MASK 0xffffffffu
@@ -25,6 +26,35 @@ inline int check_cuda(cudaError_t e, const char* what) {
 inline int post_launch(const char* what) {
   g_launches.fetch_add(1, std::memory_order_relaxed);
   return check_cuda(cudaPeekAtLastError(), what);
+}
+
+// Programmatic dependent launch (PDL).  srb_train_step launches its kernels with programmatic stream serialisation
+// (unless SRB_PDL=0): a kernel may then be scheduled while its predecessor on the stream still drains, so its launch
+// latency and CTA ramp-up overlap that tail.  Every kernel launched through launch_kernel() therefore calls pdl_wait()
+// before its first global access (read or write) of anything an earlier kernel touches, and pdl_trigger() once it runs
+// (the dependent is released only when every CTA of the grid has triggered or exited, i.e. after the last wave is
+// resident).  Outside PDL launches both instructions are no-ops.
+__device__ __forceinline__ void pdl_wait() { asm volatile("griddepcontrol.wait;" ::: "memory"); }
+__device__ __forceinline__ void pdl_trigger() { asm volatile("griddepcontrol.launch_dependents;" ::: "memory"); }
+
+bool pdl_active();  // true while srb_train_step enqueues its kernels with PDL on this thread (engine.cu)
+
+template <typename... KArgs, typename... Args>
+inline int launch_kernel(void (*kernel)(KArgs...), dim3 grid, dim3 block, size_t smem, cudaStream_t st, const char* what,
+                         Args&&... args) {
+  cudaLaunchAttribute attr[1];
+  attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
+  attr[0].val.programmaticStreamSerializationAllowed = 1;
+  cudaLaunchConfig_t cfg = {};
+  cfg.gridDim = grid;
+  cfg.blockDim = block;
+  cfg.dynamicSmemBytes = smem;
+  cfg.stream = st;
+  cfg.attrs = attr;
+  cfg.numAttrs = pdl_active() ? 1 : 0;
+  const cudaError_t e = cudaLaunchKernelEx(&cfg, kernel, std::forward<Args>(args)...);
+  g_launches.fetch_add(1, std::memory_order_relaxed);
+  return check_cuda(e, what);
 }
 
 #define SRB_REQUIRE(cond, ...)            \
@@ -57,9 +87,19 @@ struct ScatterSeg {
 };
 struct ScatterSegs {
   int count;
-  ScatterSeg s[8];
+  ScatterSeg s[16];
 };
 int scatter_segments(float* dst, int d, const ScatterSegs& segs, cudaStream_t st);
+
+// Adam step counter + bias corrections in double, like torch's Python floats (one thread)
+__device__ __forceinline__ void adam_prepare(int32_t* step, float* scalars, double lr, double b1, double b2) {
+  const int t = *step + 1;
+  *step = t;
+  const double bc1 = 1.0 - pow(b1, (double)t);
+  const double bc2 = 1.0 - pow(b2, (double)t);
+  scalars[0] = (float)(lr / bc1);
+  scalars[1] = (float)sqrt(bc2);
+}
 
 __device__ __forceinline__ float warp_sum(float v) {
 #pragma unroll

@@ -12,10 +12,31 @@
 // gradients G (<= 3B + 2B rows) are kept compact and re-scattered at every level instead of
 // being materialised as dense [N, d] tensors.  SimGCL's three encoders share A, so their
 // three backward chains collapse into one.  The last SpMM applies Adam in its epilogue.
+#include <stdlib.h>
+#include <algorithm>
 #include <mutex>
-#include "common.cuh"
+#include "spmm_args.cuh"
 
 namespace srb {
+
+// SRB_PDL=0 launches the step's kernels without programmatic dependent launch (measurement switch, same results)
+static bool pdl_enabled() {
+  static const bool on = [] {
+    const char* e = getenv("SRB_PDL");
+    return !(e && e[0] == '0');
+  }();
+  return on;
+}
+
+static thread_local bool t_pdl = false;
+bool pdl_active() { return t_pdl; }
+
+// PDL for the launches of one srb_train_step call on this thread (the sharded step and the standalone ops launch
+// without it)
+struct PdlScope {
+  PdlScope() { t_pdl = pdl_enabled(); }
+  ~PdlScope() { t_pdl = false; }
+};
 
 struct Ws {
   float* final_;  // [N,d] main encoder output
@@ -27,6 +48,7 @@ struct Ws {
   float* acc1;
   float* gd;      // dense gradient accumulator / last-layer addend
   float* rsum;    // running layer sum of the encoder being evaluated (training forwards)
+  float* seed;    // [2][N,d] backward seed tables F | G (single-chain models, see run_chain_seeded); valid at batch rows only
   float* g_emb;   // [3,B,d]
   float* g_l2;    // [3,B,d]
   float* g_nce;   // 4 x [2B,d]
@@ -47,6 +69,9 @@ struct Ws {
 };
 
 static int64_t al(int64_t x) { return (x + 255) / 256 * 256; }
+
+// models with one backward chain whose loss gradients land in the seed tables (run_chain_seeded)
+static bool seeded_chain(int model) { return model == SRB_MODEL_LIGHTGCN || model == SRB_MODEL_XSIMGCL; }
 
 static int64_t carve(const srb_step_desc* s, Ws* w, char* base) {
   const int64_t N = (int64_t)s->n_users + s->n_items, d = s->d, B = s->batch_cap;
@@ -69,6 +94,7 @@ static int64_t carve(const srb_step_desc* s, Ws* w, char* base) {
   float* f_a1 = (float*)take(graph ? nd : 0);
   float* f_gd = (float*)take(graph ? nd : 0);
   float* f_rsum = (float*)take(graph ? nd : 0);
+  float* f_seed = (float*)take(seeded_chain(s->model) ? 2 * nd : 0);
   float* f_gemb = (float*)take(3 * B * d * 4);
   float* f_gl2 = (float*)take(3 * B * d * 4);
   float* f_gnce = (float*)take(has_cl ? 4 * 2 * B * d * 4 : 0);
@@ -97,6 +123,7 @@ static int64_t carve(const srb_step_desc* s, Ws* w, char* base) {
     w->acc1 = f_a1;
     w->gd = f_gd;
     w->rsum = f_rsum;
+    w->seed = seeded_chain(s->model) ? f_seed : nullptr;  // (a zero-size take still returns the next address)
     w->g_emb = f_gemb;
     w->g_l2 = f_gl2;
     w->g_nce = f_gnce;
@@ -120,6 +147,8 @@ static int64_t carve(const srb_step_desc* s, Ws* w, char* base) {
 
 // SGL: one InfoNCE over cat(users, items) (SGL.py:120-125) needs one combined id list.
 __global__ void build_cat_idx_kernel(const int32_t* batch, int cap, int n_users, int32_t* idx_cat, int32_t* n_cat) {
+  pdl_wait();
+  pdl_trigger();
   const int nu = min(batch[1], cap), ni = min(batch[2], cap);
   const int32_t* uu = batch + SRB_BATCH_HEADER + 3 * cap;
   const int32_t* ui = uu + cap;
@@ -132,7 +161,7 @@ __global__ void build_cat_idx_kernel(const int32_t* batch, int cap, int n_users,
 // sits in a batch many times) and classified by degree on the fly for the last-layer SpMM -- split rows (their
 // chunks go to hub_work), a CTA per long row, a warp per other row; the lane-group class stays empty -- into four
 // segments of capacity 3*cap; counters[c] ends up as the size of class c, counters[4] as the number of chunks.
-// counters[0..7] and row_mask are zeroed by the caller.
+// counters[0..7] and row_mask are zeroed by step_begin_kernel.
 // With a row range [row_begin, row_begin + n_local) (row-sharded tables) only the rows of that range are listed,
 // as LOCAL row ids of the rank's CSR slice; the bitmap always covers all batch rows (global ids).
 __global__ void __launch_bounds__(256) build_batch_rows_kernel(const int32_t* batch, int cap, int n_users, const int32_t* rowptr,
@@ -140,6 +169,8 @@ __global__ void __launch_bounds__(256) build_batch_rows_kernel(const int32_t* ba
                                                                uint32_t* row_mask, int32_t* hub_first, int32_t* hub_work,
                                                                int hub_cap) {
   const int t = blockIdx.x * blockDim.x + threadIdx.x;
+  pdl_wait();
+  pdl_trigger();
   const int b = min(batch[0], cap);
   const int sec = t / cap, k = t % cap;
   if (sec >= 3 || k >= b) return;
@@ -172,7 +203,31 @@ __global__ void __launch_bounds__(256) build_batch_rows_kernel(const int32_t* ba
   }
 }
 
+// first kernel of a graph model's step: Adam's bias corrections, the batch-row counters + bitmap cleared, and (with
+// `seed`) the batch rows u, U + i, U + j of both [N, d] seed tables cleared, a float4 per thread (duplicates only repeat
+// a store).  One node instead of a kernel and two memsets.
+__global__ void __launch_bounds__(256) step_begin_kernel(int32_t* step, float* scalars, double lr, double b1, double b2, int32_t* words,
+                                                         int n_words, const int32_t* batch, int cap, int n_users, int n, int d,
+                                                         float* seed) {
+  pdl_wait();
+  pdl_trigger();
+  const int t = blockIdx.x * blockDim.x + threadIdx.x;
+  if (t == 0) adam_prepare(step, scalars, lr, b1, b2);
+  if (t < n_words) words[t] = 0;
+  if (!seed) return;
+  const int per_row = d / 4;
+  const int r = t / per_row, c = (t % per_row) * 4;
+  const int sec = r / cap, k = r % cap;
+  if (sec >= 3 || k >= min(batch[0], cap)) return;
+  const int32_t* u = batch + SRB_BATCH_HEADER;
+  const size_t row = (sec == 0) ? u[k] : n_users + u[sec * cap + k];
+  st4(seed + row * d + c, f4_zero());
+  st4(seed + ((size_t)n + row) * d + c, f4_zero());
+}
+
 __global__ void finalize_losses_kernel(const float* bpr_losses, const float* nce_losses, int n_nce, float cl_rate, float* out) {
+  pdl_wait();
+  pdl_trigger();
   float cl = 0.f;
   for (int q = 0; q < n_nce; ++q) cl += nce_losses[q];
   cl *= cl_rate;
@@ -192,7 +247,8 @@ struct Chain {
 };
 
 static int spmm_simple(const srb_step_desc* s, const srb_graph_csr* g, const float* x, float* y, const float* extra,
-                       bool adam, cudaStream_t st, const uint32_t* col_mask = nullptr) {
+                       bool adam, cudaStream_t st, const uint32_t* col_mask = nullptr, const float* seed = nullptr,
+                       const uint32_t* seed_mask = nullptr) {
   srb_spmm_desc p = {};
   p.col_mask = col_mask;
   p.rowptr = g->rowptr;
@@ -217,7 +273,11 @@ static int spmm_simple(const srb_step_desc* s, const srb_graph_csr* g, const flo
     p.beta2 = s->beta2;
     p.adam_eps = s->adam_eps;
   }
-  return srb_spmm_csr(&p, st);
+  SpmmArgs a;
+  SRB_TRY(fill_args(&p, a));
+  a.seed_mask = seed_mask;
+  a.seed = seed;
+  return launch_spmm(a, p.d, st);
 }
 
 // Horner backward of one encoder.  `gd` accumulates the E0 gradient across chains; the last
@@ -259,7 +319,7 @@ static ForkRes* fork_res(const srb_step_desc* s, ForkRes* own) {
 static ScatterSegs merged(const ScatterSegs& a, const ScatterSegs* b) {  // one launch instead of two
   ScatterSegs m = a;
   if (b)
-    for (int q = 0; q < b->count && m.count < 8; ++q) m.s[m.count++] = b->s[q];
+    for (int q = 0; q < b->count && m.count < 16; ++q) m.s[m.count++] = b->s[q];
   return m;
 }
 
@@ -291,6 +351,36 @@ static int run_chain(const srb_step_desc* s, const Ws& w, const Chain& c, bool* 
   SRB_TRY(spmm_simple(s, c.adj, x, w.gd, extra, false, st, mask));
   *gd_live = true;
   return SRB_OK;
+}
+
+// The one backward chain of LightGCN / XSimGCL, ending in Adam.  Its loss gradients are accumulated ONCE, by one
+// scatter, into two [N, d] seed tables whose batch rows step_begin_kernel cleared:
+//   F = the gradient w.r.t. the encoder's mean, which enters at levels L .. 1 (and at the ego level for LightGCN);
+//   G = what enters at the one level c of the other gradient C (layer l*, or the ego layer): C, plus F when level c
+//       also takes F.
+// The first product gathers its input (F, or G when c = L) through the batch-row bitmap, and every later level adds
+// its table in the SpMM epilogue at the rows whose batch bit is set -- no dense memset and no scatter per level.
+static int run_chain_seeded(const srb_step_desc* s, const Ws& w, const Chain& c, cudaStream_t st) {
+  const int L = s->n_layers, d = s->d, N = s->n_users + s->n_items;
+  float* F = w.seed;
+  float* G = w.seed + (size_t)N * d;
+  const ScatterSegs* cs = c.layer_cl >= 1 ? &c.cl_segs : (c.ego_segs.count ? &c.ego_segs : nullptr);
+  const int c_level = cs == &c.cl_segs ? c.layer_cl : (cs ? 0 : -1);
+  ScatterSegs sg = c.final_segs;
+  if (cs) {  // G follows F in the workspace: its segments are F's rows shifted by N
+    ScatterSegs sc = (c_level >= 1 || c.include_ego) ? merged(c.final_segs, cs) : *cs;
+    for (int q = 0; q < sc.count; ++q) sc.s[q].row_off += N;
+    sg = merged(sg, &sc);
+  }
+  SRB_TRY(scatter_segments(F, d, sg, st));
+  const float* x = c_level == L ? G : F;
+  for (int k = L - 1; k >= 1; --k) {  // acc_k = A acc_{k+1} + F (G at level c)
+    float* y = (x == w.acc0) ? w.acc1 : w.acc0;
+    SRB_TRY(spmm_simple(s, c.adj, x, y, nullptr, false, st, k == L - 1 ? w.row_mask : nullptr, c_level == k ? G : F, w.row_mask));
+    x = y;
+  }
+  const float* seed0 = c_level == 0 ? G : (c.include_ego ? F : nullptr);
+  return spmm_simple(s, c.adj, x, nullptr, nullptr, true, st, L == 1 ? w.row_mask : nullptr, seed0, w.row_mask);
 }
 
 static ScatterSeg seg(const float* src, const int32_t* rows, const int32_t* n_dev, int n, int row_off, float scale) {
@@ -402,14 +492,18 @@ extern "C" int srb_train_step(const srb_step_desc* s, void* stream) {
   const int32_t* nu_dev = hdr + 1;
   const int32_t* ni_dev = hdr + 2;
 
-  SRB_TRY(srb_adam_prepare(s->step_dev, s->scalars, s->lr, s->beta1, s->beta2, stream));
+  PdlScope pdl;
 
   // ---- forward ----
   if (s->model != SRB_MODEL_MF) {
-    SRB_TRY(check_cuda(cudaMemsetAsync(w.n_hub, 0, 32 + (size_t)((U + s->n_items + 31) / 32) * 4, st), "row mask memset"));
-    build_batch_rows_kernel<<<(3 * B + 255) / 256, 256, 0, st>>>(s->batch, B, U, s->adj.rowptr, 0, U + s->n_items, w.batch_rows, w.n_hub,
-                                                                   w.row_mask, w.hub_cap ? w.hub_first : nullptr, w.hub_work, w.hub_cap);
-    SRB_TRY(post_launch("build_batch_rows_kernel"));
+    const int n_words = 8 + (U + s->n_items + 31) / 32;  // [class counters | row bitmap]
+    const int threads = w.seed ? std::max(n_words, 3 * B * (d / 4)) : n_words;
+    SRB_TRY(launch_kernel(step_begin_kernel, (threads + 255) / 256, 256, 0, st, "step_begin_kernel", s->step_dev, s->scalars, s->lr,
+                          s->beta1, s->beta2, w.n_hub, n_words, s->batch, B, U, N, d, w.seed));
+    SRB_TRY(launch_kernel(build_batch_rows_kernel, (3 * B + 255) / 256, 256, 0, st, "build_batch_rows_kernel", s->batch, B, U, s->adj.rowptr, 0,
+                          U + s->n_items, w.batch_rows, w.n_hub, w.row_mask, w.hub_cap ? w.hub_first : nullptr, w.hub_work, w.hub_cap));
+  } else {
+    SRB_TRY(srb_adam_prepare(s->step_dev, s->scalars, s->lr, s->beta1, s->beta2, stream));
   }
   const float* table = s->params;  // table BPR gathers from
   int n_nce = 0;
@@ -506,8 +600,7 @@ extern "C" int srb_train_step(const srb_step_desc* s, void* stream) {
     SRB_TRY(srb_infonce_fwd_bwd(&q, stream));
     n_nce = 2;
   } else if (s->model == SRB_MODEL_SGL) {
-    build_cat_idx_kernel<<<8, 256, 0, st>>>(s->batch, B, U, w.idx_cat, w.n_cat);
-    SRB_TRY(post_launch("build_cat_idx_kernel"));
+    SRB_TRY(launch_kernel(build_cat_idx_kernel, 8, 256, 0, st, "build_cat_idx_kernel", s->batch, B, U, w.idx_cat, w.n_cat));
     srb_infonce_desc q = {};
     q.n_problems = 1;
     q.d = d;
@@ -520,8 +613,8 @@ extern "C" int srb_train_step(const srb_step_desc* s, void* stream) {
     n_nce = 1;
   }
   if (fk) SRB_TRY(check_cuda(cudaStreamWaitEvent(st, fk->join, 0), "join wait"));
-  finalize_losses_kernel<<<1, 1, 0, st>>>(w.bpr_losses, w.nce_losses, n_nce, s->cl_rate, s->losses);
-  SRB_TRY(post_launch("finalize_losses_kernel"));
+  SRB_TRY(launch_kernel(finalize_losses_kernel, 1, 1, 0, st, "finalize_losses_kernel", w.bpr_losses, w.nce_losses, n_nce, s->cl_rate,
+                        s->losses));
 
   // ---- backward + Adam ----
   const size_t plane = (size_t)B * d;
@@ -581,5 +674,5 @@ extern "C" int srb_train_step(const srb_step_desc* s, void* stream) {
     f.s[5] = seg(g2a, uq_u, nu_dev, B, 0, cm);
     f.s[6] = seg(g2b, uq_i, ni_dev, B, U, cm);
   }
-  return run_chain(s, w, c, &gd_live, true, st);
+  return seeded_chain(s->model) ? run_chain_seeded(s, w, c, st) : run_chain(s, w, c, &gd_live, true, st);
 }

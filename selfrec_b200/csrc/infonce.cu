@@ -69,6 +69,8 @@ __device__ __forceinline__ int nce_n(const NceProblem& p) { return p.n_dev ? min
 
 template <int D>
 __global__ void __launch_bounds__(256) nce_prep_kernel(const NceArgs a) {
+  pdl_wait();
+  pdl_trigger();
   const NceProblem& p = a.p[blockIdx.y];
   const int lane = threadIdx.x & 31;
   const int i = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
@@ -138,6 +140,8 @@ __global__ void __launch_bounds__(256) nce_prep_kernel(const NceArgs a) {
 // nce_tperm order the tensor-core kernel expects), behind dV2:
 //   hi: [V1 | V2 | V1^T | V2^T]   then lo: the same four
 __global__ void __launch_bounds__(256) nce_prep_tc_kernel(const NceArgs a) {
+  pdl_wait();
+  pdl_trigger();
   constexpr int D = 64;
   __shared__ float t1[32][D + 1], t2[32][D + 1];
   const NceProblem& p = a.p[blockIdx.y];
@@ -246,6 +250,8 @@ struct NceLseSmem {
 
 template <int D>
 __global__ void __launch_bounds__(256) nce_lse_kernel(const NceArgs a) {
+  pdl_wait();
+  pdl_trigger();
   extern __shared__ __align__(16) unsigned char smem_raw[];
   NceLseSmem<D>& sm = *reinterpret_cast<NceLseSmem<D>*>(smem_raw);
   const NceProblem& p = a.p[blockIdx.z];
@@ -320,6 +326,8 @@ struct NceGradSmem {
 
 template <int D>
 __global__ void __launch_bounds__(256) nce_grad_kernel(const NceArgs a) {
+  pdl_wait();
+  pdl_trigger();
   constexpr int CW = D / 16;  // output columns per thread in the G V products
   extern __shared__ __align__(16) unsigned char smem_raw[];
   NceGradSmem<D>& sm = *reinterpret_cast<NceGradSmem<D>*>(smem_raw);
@@ -441,6 +449,8 @@ __global__ void __launch_bounds__(256) nce_grad_kernel(const NceArgs a) {
 
 template <int D>
 __global__ void __launch_bounds__(256) nce_finish_kernel(const NceArgs a) {
+  pdl_wait();
+  pdl_trigger();
   const NceProblem& p = a.p[blockIdx.y];
   const int lane = threadIdx.x & 31;
   const int i = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
@@ -492,6 +502,8 @@ static int64_t nce_problem_floats(int np, int d) {
 // denominators l_i in part_l; dV1hat = w/(n tau l_i) dV1, both sides get the diagonal term
 // (P_ii - 1) * w/(n tau) * vhat_other in exact fp32, then the same normalisation backward as nce_finish_kernel
 __global__ void __launch_bounds__(256) nce_tc_finish_kernel(const NceArgs a) {
+  pdl_wait();
+  pdl_trigger();
   constexpr int D = 64;
   const NceProblem& p = a.p[blockIdx.y];
   const int lane = threadIdx.x & 31;
@@ -537,8 +549,7 @@ static int nce_launch_tc(const NceArgs& a, int n_problems, cudaStream_t st) {
   const int d = NT_D;
   {
     dim3 grid(np / 32, n_problems);
-    nce_prep_tc_kernel<<<grid, 256, 0, st>>>(a);
-    SRB_TRY(post_launch("nce_prep_tc_kernel"));
+    SRB_TRY(launch_kernel(nce_prep_tc_kernel, grid, 256, 0, st, "nce_prep_tc_kernel", a));
   }
   NtMaps maps;
   NtArgs t;
@@ -596,16 +607,9 @@ static int nce_launch_tc(const NceArgs& a, int n_problems, cudaStream_t st) {
     attr_done = true;
   }
   dim3 grid(row_blocks, splits, n_problems);
-  nce_tc_kernel<1><<<grid, NT_THREADS, smem, st>>>(maps, t);
-  SRB_TRY(post_launch("nce_tc_kernel<pass_a>"));
-  nce_tc_kernel<2><<<grid, NT_THREADS, smem, st>>>(maps, t);
-  SRB_TRY(post_launch("nce_tc_kernel<pass_b>"));
-  {
-    dim3 g2((np + 7) / 8, n_problems);
-    nce_tc_finish_kernel<<<g2, 256, 0, st>>>(a);
-    SRB_TRY(post_launch("nce_tc_finish_kernel"));
-  }
-  return SRB_OK;
+  SRB_TRY(launch_kernel(nce_tc_kernel<1>, grid, NT_THREADS, smem, st, "nce_tc_kernel<pass_a>", maps, t));
+  SRB_TRY(launch_kernel(nce_tc_kernel<2>, grid, NT_THREADS, smem, st, "nce_tc_kernel<pass_b>", maps, t));
+  return launch_kernel(nce_tc_finish_kernel, dim3((np + 7) / 8, n_problems), 256, 0, st, "nce_tc_finish_kernel", a);
 }
 
 template <int D>
@@ -613,8 +617,7 @@ static int nce_launch(const NceArgs& a, int n_problems, cudaStream_t st) {
   const int np = a.np;
   {
     dim3 grid((np + 7) / 8, n_problems);
-    nce_prep_kernel<D><<<grid, 256, 0, st>>>(a);
-    SRB_TRY(post_launch("nce_prep_kernel"));
+    SRB_TRY(launch_kernel(nce_prep_kernel<D>, grid, 256, 0, st, "nce_prep_kernel", a));
   }
   {
     static bool attr_done = false;
@@ -624,15 +627,12 @@ static int nce_launch(const NceArgs& a, int n_problems, cudaStream_t st) {
       attr_done = true;
     }
     dim3 grid(np / NCE_T, a.splits, n_problems);
-    nce_lse_kernel<D><<<grid, 256, sizeof(NceLseSmem<D>), st>>>(a);
-    SRB_TRY(post_launch("nce_lse_kernel"));
-    nce_grad_kernel<D><<<grid, 256, sizeof(NceGradSmem<D>), st>>>(a);
-    SRB_TRY(post_launch("nce_grad_kernel"));
+    SRB_TRY(launch_kernel(nce_lse_kernel<D>, grid, 256, sizeof(NceLseSmem<D>), st, "nce_lse_kernel", a));
+    SRB_TRY(launch_kernel(nce_grad_kernel<D>, grid, 256, sizeof(NceGradSmem<D>), st, "nce_grad_kernel", a));
   }
   {
     dim3 grid((np + 7) / 8, n_problems);
-    nce_finish_kernel<D><<<grid, 256, 0, st>>>(a);
-    SRB_TRY(post_launch("nce_finish_kernel"));
+    SRB_TRY(launch_kernel(nce_finish_kernel<D>, grid, 256, 0, st, "nce_finish_kernel", a));
   }
   return SRB_OK;
 }

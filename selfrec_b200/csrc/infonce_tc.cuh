@@ -94,6 +94,8 @@ __device__ __forceinline__ float ex2_approx(float x) {  // 2^x, flush-to-zero, 2
 // mode 1: pass A (rows = view 1)   mode 2: pass B (rows = view 2)
 template <int MODE>
 __global__ void __launch_bounds__(NT_THREADS, 1) nce_tc_kernel(const __grid_constant__ NtMaps maps, const NtArgs a) {
+  pdl_wait();
+  pdl_trigger();
   extern __shared__ __align__(1024) uint8_t nt_smem_raw[];
   uint8_t* sm = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(nt_smem_raw) + 1023) & ~(uintptr_t)1023);
   uint64_t* bars = reinterpret_cast<uint64_t*>(sm + NtSmem::bar_off);

@@ -48,6 +48,13 @@ __device__ __forceinline__ void spmm_epilogue(const SpmmArgs& a, int row, int gl
       y0 = f4_fma(a.extra_scale, *reinterpret_cast<const float4*>(a.extra + off), y0);
       y1 = f4_fma(a.extra_scale, *reinterpret_cast<const float4*>(a.extra + off + HALF), y1);
     }
+    if (a.seed && valid) {
+      const int grow = a.row_begin + row;
+      if ((__ldg(a.seed_mask + (grow >> 5)) >> (grow & 31)) & 1u) {
+        y0 = f4_add(y0, *reinterpret_cast<const float4*>(a.seed + off));
+        y1 = f4_add(y1, *reinterpret_cast<const float4*>(a.seed + off + HALF));
+      }
+    }
     if (a.noise_mode) {
       float4 n0 = f4_zero(), n1 = f4_zero();
       if (a.noise_mode == 1) {
@@ -89,8 +96,16 @@ __device__ __forceinline__ void spmm_epilogue(const SpmmArgs& a, int row, int gl
     if (a.sum_out) {
       float4 s0 = y0, s1 = y1;
       if (a.sum_in) {
-        s0 = f4_add(s0, *reinterpret_cast<const float4*>(a.sum_in + off));
-        s1 = f4_add(s1, *reinterpret_cast<const float4*>(a.sum_in + off + HALF));
+        float4 t0 = *reinterpret_cast<const float4*>(a.sum_in + off);
+        float4 t1 = *reinterpret_cast<const float4*>(a.sum_in + off + HALF);
+#pragma unroll
+        for (int j = 0; j < 3; ++j) {
+          if (!a.sum_add[j]) break;
+          t0 = f4_add(*reinterpret_cast<const float4*>(a.sum_add[j] + off), t0);
+          t1 = f4_add(*reinterpret_cast<const float4*>(a.sum_add[j] + off + HALF), t1);
+        }
+        s0 = f4_add(s0, t0);
+        s1 = f4_add(s1, t1);
       }
       s0 = f4_scale(a.sum_scale, s0);
       s1 = f4_scale(a.sum_scale, s1);
@@ -306,6 +321,8 @@ __global__ void __launch_bounds__(256) spmm_hub_kernel(const SpmmArgs a) {
   float4* stg = ASYNC ? stage + wib * SPMM_STAGE_F4 + lane : nullptr;
   const int grp = lane / LPR;
   const int gl = lane % LPR;
+  pdl_wait();
+  pdl_trigger();
   const int n_work = a.seg ? a.n_cta : (a.n_vlong_dev ? min(a.n_vlong_dev[4], a.n_work) : a.n_work);
   __shared__ float4 part[8][2][LPR];
   for (int k = blockIdx.x; k < n_work; k += gridDim.x) {
@@ -361,6 +378,8 @@ __global__ void __launch_bounds__(256) spmm_seg_warp_kernel(const SpmmArgs a) {
   const int gl = lane % LPR;
   const int warp0 = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
   const int nwarps = (gridDim.x * blockDim.x) >> 5;
+  pdl_wait();
+  pdl_trigger();
   for (int k = warp0; k < a.n_warp; k += nwarps) {
     const int w = __ldg(a.order_warp + k);
     const int beg = __ldg(a.seg + 2 * w), end = __ldg(a.seg + 2 * w + 1);
@@ -386,6 +405,8 @@ __global__ void __launch_bounds__(256) spmm_hub_finish_kernel(const SpmmArgs a) 
   const int gl = lane % LPR;
   const int warp0 = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
   const int nwarps = (gridDim.x * blockDim.x) >> 5;
+  pdl_wait();
+  pdl_trigger();
   const int n_huge = a.n_vlong_dev ? min(a.n_vlong_dev[0], a.n_rows) : a.n_huge;
   peer_wait(a.ps);  // (its epilogue may store to peers; the signal is the main kernel's, launched after this one)
   for (int vr = warp0; vr < n_huge; vr += nwarps) {
@@ -417,6 +438,8 @@ __global__ void __launch_bounds__(256) spmm_csr_kernel(const SpmmArgs a) {
   const int warp0 = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
   const int nwarps = (gridDim.x * blockDim.x) >> 5;
 
+  pdl_wait();
+  pdl_trigger();
   peer_wait(a.ps);
   // (the split rows -- the first n_huge entries of the list -- belong to spmm_hub_kernel / spmm_hub_finish_kernel)
   int n_vlong = a.n_vlong, n_long = a.n_long, n_short = a.n_rows - a.n_huge - a.n_vlong - a.n_long;
@@ -590,6 +613,8 @@ __global__ void __launch_bounds__(256) rows_epilogue_kernel(const SpmmArgs a) {
   const int warp0 = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
   const int nwarps = (gridDim.x * blockDim.x) >> 5;
   const int n_items = (a.n_rows + RPW - 1) / RPW;
+  pdl_wait();
+  pdl_trigger();
   for (int item = warp0; item < n_items; item += nwarps) {
     const int row = item * RPW + grp;
     const bool valid = row < a.n_rows;
@@ -611,12 +636,11 @@ int launch_rows_epilogue(const SpmmArgs& a, int d, cudaStream_t st) {
   if (blocks > cap) blocks = cap;
   if (blocks < 1) blocks = 1;
   switch (d) {
-    case 32: rows_epilogue_kernel<32><<<(int)blocks, 256, 0, st>>>(a); break;
-    case 64: rows_epilogue_kernel<64><<<(int)blocks, 256, 0, st>>>(a); break;
-    case 128: rows_epilogue_kernel<128><<<(int)blocks, 256, 0, st>>>(a); break;
+    case 32: return launch_kernel(rows_epilogue_kernel<32>, (int)blocks, 256, 0, st, "rows_epilogue_kernel", a);
+    case 64: return launch_kernel(rows_epilogue_kernel<64>, (int)blocks, 256, 0, st, "rows_epilogue_kernel", a);
+    case 128: return launch_kernel(rows_epilogue_kernel<128>, (int)blocks, 256, 0, st, "rows_epilogue_kernel", a);
     default: set_error("rows_epilogue: unsupported d=%d (32, 64, 128)", d); return SRB_ERR_ARG;
   }
-  return post_launch("rows_epilogue_kernel");
 }
 
 int launch_reduce_rows(const SpmmArgs& a, const ReduceArgs& r, int d, cudaStream_t st) {
@@ -636,26 +660,24 @@ int launch_reduce_rows(const SpmmArgs& a, const ReduceArgs& r, int d, cudaStream
 }
 
 template <int D, bool M, bool AS>
-static void launch_spmm_dma(const SpmmArgs& a, int hub_blocks, int blocks, cudaStream_t st) {
+static int launch_spmm_dma(const SpmmArgs& a, int hub_blocks, int blocks, cudaStream_t st) {
   if (hub_blocks > 0) {
     if (a.seg && a.n_warp > 0) {
       const int wb = max(1, min((a.n_warp + 7) / 8, blocks));
-      spmm_seg_warp_kernel<D, M, AS><<<wb, 256, 0, st>>>(a);
-      g_launches.fetch_add(1, std::memory_order_relaxed);
+      SRB_TRY(launch_kernel(spmm_seg_warp_kernel<D, M, AS>, wb, 256, 0, st, "spmm_seg_warp_kernel", a));
     }
-    spmm_hub_kernel<D, M, AS><<<hub_blocks, 256, 0, st>>>(a);
+    SRB_TRY(launch_kernel(spmm_hub_kernel<D, M, AS>, hub_blocks, 256, 0, st, "spmm_hub_kernel", a));
     const int nh = a.n_vlong_dev ? a.n_rows : a.n_huge;  // (device-counted lists: the capacity)
-    spmm_hub_finish_kernel<D><<<max(1, min((nh + 7) / 8, hub_blocks)), 256, 0, st>>>(a);
-    g_launches.fetch_add(2, std::memory_order_relaxed);
+    SRB_TRY(launch_kernel(spmm_hub_finish_kernel<D>, max(1, min((nh + 7) / 8, hub_blocks)), 256, 0, st, "spmm_hub_finish_kernel", a));
   }
-  spmm_csr_kernel<D, M, AS><<<blocks, 256, 0, st>>>(a);
+  return launch_kernel(spmm_csr_kernel<D, M, AS>, blocks, 256, 0, st, "spmm_csr_kernel", a);
 }
 
 template <int D>
-static void launch_spmm_d(const SpmmArgs& a, int hub_blocks, int blocks, cudaStream_t st) {
-  if (a.col_mask != nullptr) launch_spmm_dma<D, true, false>(a, hub_blocks, blocks, st);
-  else if (D >= 64 && a.async_stage) launch_spmm_dma<D, false, (D >= 64)>(a, hub_blocks, blocks, st);
-  else launch_spmm_dma<D, false, false>(a, hub_blocks, blocks, st);
+static int launch_spmm_d(const SpmmArgs& a, int hub_blocks, int blocks, cudaStream_t st) {
+  if (a.col_mask != nullptr) return launch_spmm_dma<D, true, false>(a, hub_blocks, blocks, st);
+  if (D >= 64 && a.async_stage) return launch_spmm_dma<D, false, (D >= 64)>(a, hub_blocks, blocks, st);
+  return launch_spmm_dma<D, false, false>(a, hub_blocks, blocks, st);
 }
 
 int launch_spmm(const SpmmArgs& a, int d, cudaStream_t st) {
@@ -672,12 +694,11 @@ int launch_spmm(const SpmmArgs& a, int d, cudaStream_t st) {
   long long hub_blocks = a.seg ? (a.n_cta > 0 ? a.n_cta : (a.n_work > 0 ? 1 : 0)) : a.n_work;  // (device-counted lists: the capacity)
   if (hub_blocks > cap) hub_blocks = cap;
   switch (d) {
-    case 32: launch_spmm_d<32>(a, (int)hub_blocks, (int)blocks, st); break;
-    case 64: launch_spmm_d<64>(a, (int)hub_blocks, (int)blocks, st); break;
-    case 128: launch_spmm_d<128>(a, (int)hub_blocks, (int)blocks, st); break;
+    case 32: return launch_spmm_d<32>(a, (int)hub_blocks, (int)blocks, st);
+    case 64: return launch_spmm_d<64>(a, (int)hub_blocks, (int)blocks, st);
+    case 128: return launch_spmm_d<128>(a, (int)hub_blocks, (int)blocks, st);
     default: set_error("spmm: unsupported d=%d (32, 64, 128)", d); return SRB_ERR_ARG;
   }
-  return post_launch("spmm_csr_kernel");
 }
 
 // SRB_SPMM_ASYNC=1 stages every second gather sub-batch through cp.async + shared memory (measurement switch; results
@@ -731,6 +752,8 @@ int fill_args(const srb_spmm_desc* d, SpmmArgs& a) {
   a.Y = d->Y;
   a.extra = d->extra;
   a.extra_scale = d->extra_scale;
+  a.seed_mask = nullptr;
+  a.seed = nullptr;
   a.noise_mode = d->noise_mode;
   a.noise = d->noise;
   a.eps = d->eps;
@@ -738,6 +761,7 @@ int fill_args(const srb_spmm_desc* d, SpmmArgs& a) {
   a.poff = make_uint2((uint32_t)d->philox_offset, (uint32_t)(d->philox_offset >> 32));
   a.pstep = d->philox_step_dev;
   a.sum_in = d->sum_in;
+  a.sum_add[0] = a.sum_add[1] = a.sum_add[2] = nullptr;
   a.sum_out = d->sum_out;
   a.sum_scale = d->sum_scale;
   a.ap = d->adam_p;
@@ -808,6 +832,24 @@ extern "C" int srb_encoder_forward(const srb_encoder_desc* e, void* stream) {
     x = e->x1;
     k0 = 1;
   }
+  const bool last_on_rows = e->last_rows && e->n_last_rows > 0 && !(cl_hit && e->layer_cl == L);
+  // Layer mean on the batch rows only: when the last layer runs on the listed rows and every earlier layer output is
+  // still in a buffer of its own (cl_out, work0/1, x1: L <= 3), the full-size layers keep no running sum; the last
+  // layer's epilogue adds E0 (when the ego layer counts), E1, ..., E(L-1) at its rows, in the order the running sum
+  // would have (((E0 + E1) + E2) + E3), so the mean is bit-identical.
+  const float* src[4];
+  int n_src = 0;
+  bool live = true;
+  if (e->include_ego) src[n_src++] = e->E0;
+  const float* px = e->E0;
+  for (int k = 0; k < L - 1 && live; ++k) {  // where the loop below leaves the output of layer k + 1
+    const float* py = (k == 0 && e->x1) ? e->x1 : (cl_hit && k == e->layer_cl - 1) ? e->cl_out : (px == e->work0 ? e->work1 : e->work0);
+    for (int j = 0; j < n_src; ++j) live = live && src[j] != py;
+    live = live && n_src < 4;
+    if (live) src[n_src++] = py;
+    px = py;
+  }
+  const bool batch_mean = last_on_rows && live;
   for (int k = k0; k < L; ++k) {
     srb_spmm_desc s = {};
     s.rowptr = e->rowptr;
@@ -834,9 +876,10 @@ extern "C" int srb_encoder_forward(const srb_encoder_desc* e, void* stream) {
     s.philox_step_dev = e->philox_step_dev;
     // running sum lives in final_out; layer 1 seeds it (with E0 when the ego layer counts)
     s.sum_in = (k == 0) ? (e->include_ego ? e->E0 : nullptr) : ((k == 1 && e->x1) ? e->x1 : e->final_out);
-    s.sum_out = e->final_out;
+    s.sum_out = (batch_mean && !last) ? nullptr : e->final_out;
     s.sum_scale = last ? inv : 1.0f;
-    if (last && e->last_rows && e->n_last_rows > 0 && !(cl_hit && k == e->layer_cl - 1)) {
+    if (batch_mean && last) s.sum_in = n_src ? src[0] : nullptr;
+    if (last && last_on_rows) {
       // only the listed rows of the final mean are consumed: one warp per listed row
       s.row_order = e->last_rows;
       s.n_rows = e->n_last_rows;
@@ -853,7 +896,11 @@ extern "C" int srb_encoder_forward(const srb_encoder_desc* e, void* stream) {
       s.Y = nullptr;
       s.sum_out = e->last_rows_out;  // out of place: duplicates in the list stay idempotent
     }
-    SRB_TRY(srb_spmm_csr(&s, stream));
+    srb::SpmmArgs a;
+    SRB_TRY(srb::fill_args(&s, a));
+    if (batch_mean && last)
+      for (int j = 1; j < n_src; ++j) a.sum_add[j - 1] = src[j];
+    SRB_TRY(srb::launch_spmm(a, s.d, st));
     x = y;
   }
   return SRB_OK;

@@ -91,6 +91,10 @@ struct SpmmArgs {
   float* Y;
   const float* extra;
   float extra_scale;
+  // optional backward seed table (engine.cu, run_chain_seeded): y += seed[row] where seed_mask has the row's bit; the
+  // table holds nothing elsewhere
+  const uint32_t* seed_mask;
+  const float* seed;
   int32_t noise_mode;
   const float* noise;
   float eps;
@@ -98,6 +102,7 @@ struct SpmmArgs {
   uint2 poff;
   const int32_t* pstep;
   const float* sum_in;
+  const float* sum_add[3];  // optional: earlier layer outputs, added onto sum_in in this order before the row's own value
   float* sum_out;
   float sum_scale;
   float* ap;
