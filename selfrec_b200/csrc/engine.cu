@@ -9,9 +9,10 @@
 // SimGCL/XSimGCL noise has zero gradient (sign() and the noise are constants):
 //   final = c * sum_k A^k E0   =>   dE0 = c * sum_k A^k G      (A symmetric)
 // evaluated by Horner's rule with L SpMMs and no saved activations; the row-sparse loss
-// gradients G (<= 3B + 2B rows) are kept compact and re-scattered at every level instead of
-// being materialised as dense [N, d] tensors.  SimGCL's three encoders share A, so their
-// three backward chains collapse into one.  The last SpMM applies Adam in its epilogue.
+// gradients G (<= 3B + 2B rows) are scattered once into [N, d] seed tables that hold data only
+// at the batch rows, and each Horner level adds its table in the SpMM epilogue (run_chain).
+// SimGCL's three encoders share A, so their three backward chains collapse into one.  The last
+// SpMM applies Adam in its epilogue.
 #include <stdlib.h>
 #include <algorithm>
 #include <mutex>
@@ -46,9 +47,10 @@ struct Ws {
   float* work1;
   float* acc0;
   float* acc1;
-  float* gd;      // dense gradient accumulator / last-layer addend
+  float* gd;      // [N,d] SimGCL: view 2's first layer (L >= 2); SGL: the sum of the two view chains
   float* rsum;    // running layer sum of the encoder being evaluated (training forwards)
-  float* seed;    // [2][N,d] backward seed tables F | G (single-chain models, see run_chain_seeded); valid at batch rows only
+  float* seed;    // [n_seed][N,d] backward seed tables (see run_chain); valid at batch rows only
+  int32_t n_seed; // LightGCN, XSimGCL: F | G; SimGCL: F; SGL: F of the encoders on adj_view[0] | adj_view[1] | adj
   float* g_emb;   // [3,B,d]
   float* g_l2;    // [3,B,d]
   float* g_nce;   // 4 x [2B,d]
@@ -70,9 +72,6 @@ struct Ws {
 
 static int64_t al(int64_t x) { return (x + 255) / 256 * 256; }
 
-// models with one backward chain whose loss gradients land in the seed tables (run_chain_seeded)
-static bool seeded_chain(int model) { return model == SRB_MODEL_LIGHTGCN || model == SRB_MODEL_XSIMGCL; }
-
 static int64_t carve(const srb_step_desc* s, Ws* w, char* base) {
   const int64_t N = (int64_t)s->n_users + s->n_items, d = s->d, B = s->batch_cap;
   const int64_t nd = al(N * d * 4);
@@ -85,16 +84,9 @@ static int64_t carve(const srb_step_desc* s, Ws* w, char* base) {
   const bool graph = s->model != SRB_MODEL_MF;
   const bool two_views = s->model == SRB_MODEL_SIMGCL || s->model == SRB_MODEL_SGL;
   const bool has_cl = s->model == SRB_MODEL_XSIMGCL || two_views;
-  float* f_final = (float*)take(graph ? nd : 0);
-  float* f_cl = (float*)take(has_cl ? nd : 0);
-  float* f_v2 = (float*)take(two_views ? nd : 0);
-  float* f_w0 = (float*)take(graph ? nd : 0);
-  float* f_w1 = (float*)take(graph ? nd : 0);
-  float* f_a0 = (float*)take(nd);
-  float* f_a1 = (float*)take(graph ? nd : 0);
-  float* f_gd = (float*)take(graph ? nd : 0);
-  float* f_rsum = (float*)take(graph ? nd : 0);
-  float* f_seed = (float*)take(seeded_chain(s->model) ? 2 * nd : 0);
+  const int n_seed = s->model == SRB_MODEL_SGL ? 3 : (s->model == SRB_MODEL_SIMGCL ? 1 : (graph ? 2 : 0));
+  // the small per-step buffers first, at offsets that do not depend on which [N, d] tables the model has: behind the
+  // tables, one table less moved them and made the yelp2018 XSimGCL step 0.7 us slower (H100 80GB HBM3, 700 W)
   float* f_gemb = (float*)take(3 * B * d * 4);
   float* f_gl2 = (float*)take(3 * B * d * 4);
   float* f_gnce = (float*)take(has_cl ? 4 * 2 * B * d * 4 : 0);
@@ -113,6 +105,16 @@ static int64_t carve(const srb_step_desc* s, Ws* w, char* base) {
   float* f_hpart = (float*)take(hub_cap * d * 4);
   const int64_t nws = has_cl ? srb_infonce_workspace_bytes((int32_t)(2 * B), (int32_t)d, 2) : 0;
   void* v_nws = take(nws);
+  float* f_final = (float*)take(graph ? nd : 0);
+  float* f_cl = (float*)take(has_cl ? nd : 0);
+  float* f_v2 = (float*)take(two_views ? nd : 0);
+  float* f_w0 = (float*)take(graph ? nd : 0);
+  float* f_w1 = (float*)take(graph ? nd : 0);
+  float* f_a0 = (float*)take(nd);
+  float* f_a1 = (float*)take(graph ? nd : 0);
+  float* f_gd = (float*)take(two_views ? nd : 0);
+  float* f_rsum = (float*)take(graph ? nd : 0);
+  float* f_seed = (float*)take(n_seed * nd);
   if (w) {
     w->final_ = f_final;
     w->cl = f_cl;
@@ -123,7 +125,8 @@ static int64_t carve(const srb_step_desc* s, Ws* w, char* base) {
     w->acc1 = f_a1;
     w->gd = f_gd;
     w->rsum = f_rsum;
-    w->seed = seeded_chain(s->model) ? f_seed : nullptr;  // (a zero-size take still returns the next address)
+    w->seed = f_seed;
+    w->n_seed = n_seed;
     w->g_emb = f_gemb;
     w->g_l2 = f_gl2;
     w->g_nce = f_gnce;
@@ -203,26 +206,24 @@ __global__ void __launch_bounds__(256) build_batch_rows_kernel(const int32_t* ba
   }
 }
 
-// first kernel of a graph model's step: Adam's bias corrections, the batch-row counters + bitmap cleared, and (with
-// `seed`) the batch rows u, U + i, U + j of both [N, d] seed tables cleared, a float4 per thread (duplicates only repeat
-// a store).  One node instead of a kernel and two memsets.
+// first kernel of a graph model's step: Adam's bias corrections, the batch-row counters + bitmap cleared, and the batch
+// rows u, U + i, U + j of the n_seed [N, d] seed tables cleared, a float4 per thread (duplicates only repeat a store).
+// One node instead of a kernel and two memsets.
 __global__ void __launch_bounds__(256) step_begin_kernel(int32_t* step, float* scalars, double lr, double b1, double b2, int32_t* words,
                                                          int n_words, const int32_t* batch, int cap, int n_users, int n, int d,
-                                                         float* seed) {
+                                                         float* seed, int n_seed) {
   pdl_wait();
   pdl_trigger();
   const int t = blockIdx.x * blockDim.x + threadIdx.x;
   if (t == 0) adam_prepare(step, scalars, lr, b1, b2);
   if (t < n_words) words[t] = 0;
-  if (!seed) return;
   const int per_row = d / 4;
   const int r = t / per_row, c = (t % per_row) * 4;
   const int sec = r / cap, k = r % cap;
   if (sec >= 3 || k >= min(batch[0], cap)) return;
   const int32_t* u = batch + SRB_BATCH_HEADER;
   const size_t row = (sec == 0) ? u[k] : n_users + u[sec * cap + k];
-  st4(seed + row * d + c, f4_zero());
-  st4(seed + ((size_t)n + row) * d + c, f4_zero());
+  for (int q = 0; q < n_seed; ++q) st4(seed + ((size_t)q * n + row) * d + c, f4_zero());
 }
 
 __global__ void finalize_losses_kernel(const float* bpr_losses, const float* nce_losses, int n_nce, float cl_rate, float* out) {
@@ -236,15 +237,6 @@ __global__ void finalize_losses_kernel(const float* bpr_losses, const float* nce
   out[2] = cl;
   out[3] = bpr_losses[0] + bpr_losses[1] + cl;
 }
-
-struct Chain {
-  const srb_graph_csr* adj;
-  ScatterSegs final_segs;  // gradient w.r.t. the encoder's mean output (scale folded in)
-  ScatterSegs cl_segs;     // gradient w.r.t. the output of layer `layer_cl`
-  ScatterSegs ego_segs;    // gradient that lands on E0 directly
-  int layer_cl;            // 1..L, or 0 when none / at the ego layer
-  bool include_ego;
-};
 
 static int spmm_simple(const srb_step_desc* s, const srb_graph_csr* g, const float* x, float* y, const float* extra,
                        bool adam, cudaStream_t st, const uint32_t* col_mask = nullptr, const float* seed = nullptr,
@@ -280,8 +272,6 @@ static int spmm_simple(const srb_step_desc* s, const srb_graph_csr* g, const flo
   return launch_spmm(a, p.d, st);
 }
 
-// Horner backward of one encoder.  `gd` accumulates the E0 gradient across chains; the last
-// chain applies Adam.  gd_live says whether gd already holds earlier chains' contributions.
 // BPR + L2 and InfoNCE only read the encoder outputs and write disjoint buffers: the step forks BPR onto a
 // side stream (event dependencies, so a stream capture records the fork and join) and joins before the
 // losses are combined.
@@ -316,71 +306,26 @@ static ForkRes* fork_res(const srb_step_desc* s, ForkRes* own) {
   return &r;
 }
 
-static ScatterSegs merged(const ScatterSegs& a, const ScatterSegs* b) {  // one launch instead of two
-  ScatterSegs m = a;
-  if (b)
-    for (int q = 0; q < b->count && m.count < 16; ++q) m.s[m.count++] = b->s[q];
-  return m;
-}
-
-static int run_chain(const srb_step_desc* s, const Ws& w, const Chain& c, bool* gd_live, bool last, cudaStream_t st) {
-  const int L = s->n_layers, d = s->d;
-  const size_t bytes = (size_t)(s->n_users + s->n_items) * d * 4;
-  // seed: gradient w.r.t. the output of layer L
-  SRB_TRY(check_cuda(cudaMemsetAsync(w.acc0, 0, bytes, st), "chain memset"));
-  SRB_TRY(scatter_segments(w.acc0, d, merged(c.final_segs, c.layer_cl == L ? &c.cl_segs : nullptr), st));
-  float* x = w.acc0;
-  for (int k = L - 1; k >= 1; --k) {  // acc_k = A acc_{k+1} + (direct gradient of layer k)
+// The Horner backward chain of one encoder on graph g.  Its loss gradients were scattered beforehand into [N, d] seed
+// tables whose batch rows step_begin_kernel cleared:
+//   F = the gradient w.r.t. the encoder's mean, which enters at levels L .. 1 (and at the ego level with include_ego);
+//   G (optional, else nullptr with g_level = -1) = what enters at level g_level instead of F (XSimGCL's layer l* or
+//       ego-layer gradient, LightGCN's L2 gradient on E0), plus F when that level also takes F.
+// The first product gathers its input (F, or G when g_level = L) through the batch-row bitmap, and every later level
+// adds its table in the SpMM epilogue at the rows whose batch bit is set -- no dense memset and no scatter per level.
+// The last product adds the dense `extra` (may be nullptr) and applies Adam, or with `out` stores into it instead
+// (out == extra is allowed: each row reads its addend before it stores).
+static int run_chain(const srb_step_desc* s, const Ws& w, const srb_graph_csr* g, const float* F, const float* G, int g_level,
+                     bool include_ego, float* out, const float* extra, cudaStream_t st) {
+  const int L = s->n_layers;
+  const float* x = g_level == L ? G : F;
+  for (int k = L - 1; k >= 1; --k) {  // acc_k = A acc_{k+1} + F (G at level g_level)
     float* y = (x == w.acc0) ? w.acc1 : w.acc0;
-    SRB_TRY(spmm_simple(s, c.adj, x, y, nullptr, false, st, k == L - 1 ? w.row_mask : nullptr));  // seed: batch rows only
-    SRB_TRY(scatter_segments(y, d, merged(c.final_segs, c.layer_cl == k ? &c.cl_segs : nullptr), st));
+    SRB_TRY(spmm_simple(s, g, x, y, nullptr, false, st, k == L - 1 ? w.row_mask : nullptr, g_level == k ? G : F, w.row_mask));
     x = y;
   }
-  const bool ego_add = (c.include_ego && c.final_segs.count) || c.ego_segs.count;
-  if (ego_add && !*gd_live) {
-    SRB_TRY(check_cuda(cudaMemsetAsync(w.gd, 0, bytes, st), "chain memset gd"));
-    *gd_live = true;
-  }
-  if (ego_add) {
-    if (c.include_ego) SRB_TRY(scatter_segments(w.gd, d, merged(c.final_segs, &c.ego_segs), st));
-    else SRB_TRY(scatter_segments(w.gd, d, c.ego_segs, st));
-  }
-  const float* extra = *gd_live ? w.gd : nullptr;
-  const uint32_t* mask = (L == 1) ? w.row_mask : nullptr;
-  if (last) return spmm_simple(s, c.adj, x, nullptr, extra, true, st, mask);
-  SRB_TRY(spmm_simple(s, c.adj, x, w.gd, extra, false, st, mask));
-  *gd_live = true;
-  return SRB_OK;
-}
-
-// The one backward chain of LightGCN / XSimGCL, ending in Adam.  Its loss gradients are accumulated ONCE, by one
-// scatter, into two [N, d] seed tables whose batch rows step_begin_kernel cleared:
-//   F = the gradient w.r.t. the encoder's mean, which enters at levels L .. 1 (and at the ego level for LightGCN);
-//   G = what enters at the one level c of the other gradient C (layer l*, or the ego layer): C, plus F when level c
-//       also takes F.
-// The first product gathers its input (F, or G when c = L) through the batch-row bitmap, and every later level adds
-// its table in the SpMM epilogue at the rows whose batch bit is set -- no dense memset and no scatter per level.
-static int run_chain_seeded(const srb_step_desc* s, const Ws& w, const Chain& c, cudaStream_t st) {
-  const int L = s->n_layers, d = s->d, N = s->n_users + s->n_items;
-  float* F = w.seed;
-  float* G = w.seed + (size_t)N * d;
-  const ScatterSegs* cs = c.layer_cl >= 1 ? &c.cl_segs : (c.ego_segs.count ? &c.ego_segs : nullptr);
-  const int c_level = cs == &c.cl_segs ? c.layer_cl : (cs ? 0 : -1);
-  ScatterSegs sg = c.final_segs;
-  if (cs) {  // G follows F in the workspace: its segments are F's rows shifted by N
-    ScatterSegs sc = (c_level >= 1 || c.include_ego) ? merged(c.final_segs, cs) : *cs;
-    for (int q = 0; q < sc.count; ++q) sc.s[q].row_off += N;
-    sg = merged(sg, &sc);
-  }
-  SRB_TRY(scatter_segments(F, d, sg, st));
-  const float* x = c_level == L ? G : F;
-  for (int k = L - 1; k >= 1; --k) {  // acc_k = A acc_{k+1} + F (G at level c)
-    float* y = (x == w.acc0) ? w.acc1 : w.acc0;
-    SRB_TRY(spmm_simple(s, c.adj, x, y, nullptr, false, st, k == L - 1 ? w.row_mask : nullptr, c_level == k ? G : F, w.row_mask));
-    x = y;
-  }
-  const float* seed0 = c_level == 0 ? G : (c.include_ego ? F : nullptr);
-  return spmm_simple(s, c.adj, x, nullptr, nullptr, true, st, L == 1 ? w.row_mask : nullptr, seed0, w.row_mask);
+  const float* seed0 = g_level == 0 ? G : (include_ego ? F : nullptr);
+  return spmm_simple(s, g, x, out, extra, out == nullptr, st, L == 1 ? w.row_mask : nullptr, seed0, w.row_mask);
 }
 
 static ScatterSeg seg(const float* src, const int32_t* rows, const int32_t* n_dev, int n, int row_off, float scale) {
@@ -497,9 +442,9 @@ extern "C" int srb_train_step(const srb_step_desc* s, void* stream) {
   // ---- forward ----
   if (s->model != SRB_MODEL_MF) {
     const int n_words = 8 + (U + s->n_items + 31) / 32;  // [class counters | row bitmap]
-    const int threads = w.seed ? std::max(n_words, 3 * B * (d / 4)) : n_words;
+    const int threads = std::max(n_words, 3 * B * (d / 4));
     SRB_TRY(launch_kernel(step_begin_kernel, (threads + 255) / 256, 256, 0, st, "step_begin_kernel", s->step_dev, s->scalars, s->lr,
-                          s->beta1, s->beta2, w.n_hub, n_words, s->batch, B, U, N, d, w.seed));
+                          s->beta1, s->beta2, w.n_hub, n_words, s->batch, B, U, N, d, w.seed, w.n_seed));
     SRB_TRY(launch_kernel(build_batch_rows_kernel, (3 * B + 255) / 256, 256, 0, st, "build_batch_rows_kernel", s->batch, B, U, s->adj.rowptr, 0,
                           U + s->n_items, w.batch_rows, w.n_hub, w.row_mask, w.hub_cap ? w.hub_first : nullptr, w.hub_work, w.hub_cap));
   } else {
@@ -524,7 +469,7 @@ extern "C" int srb_train_step(const srb_step_desc* s, void* stream) {
       SRB_REQUIRE(s->noise_mode != 1 || s->noise, "step: noise tensor missing");
       if (L >= 2) {
         // layer 1 of the three encoders is the same product A * E0 (SimGCL.py:85); only the noise added to it differs
-        // (:87-88).  It is evaluated once; acc0 / acc1 / gd belong to the backward pass and are free until then.
+        // (:87-88).  It is evaluated once; acc0 / acc1 belong to the backward pass and are free until then.
         SRB_TRY(spmm_simple(s, &s->adj, s->params, w.acc0, nullptr, false, st));
         SRB_TRY(perturb_rows(s, w.acc0, w.acc1, 0, st));
         SRB_TRY(perturb_rows(s, w.acc0, w.gd, 1, st));
@@ -630,49 +575,57 @@ extern "C" int srb_train_step(const srb_step_desc* s, void* stream) {
     return srb_adam_step(s->params, s->adam_m, s->adam_v, w.acc0, (int64_t)N * d, s->scalars, s->beta1, s->beta2, s->adam_eps,
                          stream);
   }
-  const float cm = 1.f / (float)((s->model == SRB_MODEL_LIGHTGCN || s->model == SRB_MODEL_SGL) ? L + 1 : L);
-  bool gd_live = false;
-  if (s->model == SRB_MODEL_SGL) {
-    // two view encoders on their own graphs, then the main chain with Adam
-    for (int v = 0; v < 2; ++v) {
-      Chain c = {};
-      c.adj = &s->adj_view[v];
-      c.include_ego = true;
-      c.final_segs.count = 1;
-      c.final_segs.s[0] = seg(v == 0 ? g1a : g2a, w.idx_cat, w.n_cat, 2 * B, 0, cm);
-      SRB_TRY(run_chain(s, w, c, &gd_live, false, st));
-    }
+  const bool ego = s->model == SRB_MODEL_LIGHTGCN || s->model == SRB_MODEL_SGL;
+  const float cm = 1.f / (float)(ego ? L + 1 : L);
+  // one scatter fills every seed table: table t's rows are shifted by t * N
+  auto seed_table = [&](int t) { return w.seed + (size_t)t * N * d; };
+  ScatterSegs sg = {};
+  auto add = [&](int t, const float* src, const int32_t* rows, const int32_t* n_dev, int n, int row_off, float scale) {
+    sg.s[sg.count++] = seg(src, rows, n_dev, n, t * N + row_off, scale);
+  };
+  auto add_bpr = [&](int t, const float* g, float scale) {  // rows u, U + i, U + j
+    add(t, g, u_idx, b_dev, B, 0, scale);
+    add(t, g + plane, i_idx, b_dev, B, U, scale);
+    add(t, g + 2 * plane, j_idx, b_dev, B, U, scale);
+  };
+  auto add_nce = [&](int t, const float* gu, const float* gi, float scale) {  // unique batch users, U + unique items
+    add(t, gu, uq_u, nu_dev, B, 0, scale);
+    add(t, gi, uq_i, ni_dev, B, U, scale);
+  };
+  int g_level = -1;  // LightGCN, XSimGCL: the level where table 1 (G) enters instead of F
+  switch (s->model) {
+    case SRB_MODEL_LIGHTGCN:  // the L2 term regularises the raw E0: G = F + its gradient at the ego level
+      add_bpr(0, w.g_emb, cm);
+      add_bpr(1, w.g_emb, cm);
+      add_bpr(1, w.g_l2, 1.f);
+      g_level = 0;
+      break;
+    case SRB_MODEL_XSIMGCL:
+      // view 1 = final (mean) rows, view 2 = layer l* output (XSimGCL.py:45-50); G = view 2's gradient, plus F unless
+      // l* is the ego layer, which the mean leaves out
+      g_level = (s->layer_cl >= 1 && s->layer_cl <= L) ? s->layer_cl : 0;
+      for (int t = 0; t < (g_level ? 2 : 1); ++t) {
+        add_bpr(t, w.g_emb, cm);
+        add_nce(t, g1a, g1b, cm);
+      }
+      add_nce(1, g2a, g2b, 1.f);
+      break;
+    case SRB_MODEL_SIMGCL:  // all three encoders are the same linear map of E0: one merged chain
+      add_bpr(0, w.g_emb, cm);
+      add_nce(0, g1a, g1b, cm);
+      add_nce(0, g2a, g2b, cm);
+      break;
+    case SRB_MODEL_SGL:  // a table per encoder graph: adj_view[0], adj_view[1], adj
+      add(0, g1a, w.idx_cat, w.n_cat, 2 * B, 0, cm);
+      add(1, g2a, w.idx_cat, w.n_cat, 2 * B, 0, cm);
+      add_bpr(2, w.g_emb, cm);
+      break;
   }
-  Chain c = {};
-  c.adj = &s->adj;
-  c.include_ego = (s->model == SRB_MODEL_LIGHTGCN || s->model == SRB_MODEL_SGL);
-  ScatterSegs& f = c.final_segs;
-  f.count = 3;
-  f.s[0] = seg(w.g_emb, u_idx, b_dev, B, 0, cm);
-  f.s[1] = seg(w.g_emb + plane, i_idx, b_dev, B, U, cm);
-  f.s[2] = seg(w.g_emb + 2 * plane, j_idx, b_dev, B, U, cm);
-  if (s->model == SRB_MODEL_LIGHTGCN) {
-    c.ego_segs.count = 3;
-    c.ego_segs.s[0] = seg(w.g_l2, u_idx, b_dev, B, 0, 1.f);
-    c.ego_segs.s[1] = seg(w.g_l2 + plane, i_idx, b_dev, B, U, 1.f);
-    c.ego_segs.s[2] = seg(w.g_l2 + 2 * plane, j_idx, b_dev, B, U, 1.f);
-  } else if (s->model == SRB_MODEL_XSIMGCL) {
-    // view 1 = final (mean) rows, view 2 = layer l* output (XSimGCL.py:45-50)
-    f.count = 5;
-    f.s[3] = seg(g1a, uq_u, nu_dev, B, 0, cm);
-    f.s[4] = seg(g1b, uq_i, ni_dev, B, U, cm);
-    ScatterSegs& cs = (s->layer_cl >= 1 && s->layer_cl <= L) ? c.cl_segs : c.ego_segs;
-    cs.count = 2;
-    cs.s[0] = seg(g2a, uq_u, nu_dev, B, 0, 1.f);
-    cs.s[1] = seg(g2b, uq_i, ni_dev, B, U, 1.f);
-    c.layer_cl = (s->layer_cl >= 1 && s->layer_cl <= L) ? s->layer_cl : 0;
-  } else if (s->model == SRB_MODEL_SIMGCL) {
-    // all three encoders are the same linear map of E0: one merged chain
-    f.count = 7;
-    f.s[3] = seg(g1a, uq_u, nu_dev, B, 0, cm);
-    f.s[4] = seg(g1b, uq_i, ni_dev, B, U, cm);
-    f.s[5] = seg(g2a, uq_u, nu_dev, B, 0, cm);
-    f.s[6] = seg(g2b, uq_i, ni_dev, B, U, cm);
-  }
-  return seeded_chain(s->model) ? run_chain_seeded(s, w, c, st) : run_chain(s, w, c, &gd_live, true, st);
+  SRB_TRY(scatter_segments(w.seed, d, sg, st));
+  if (s->model != SRB_MODEL_SGL)
+    return run_chain(s, w, &s->adj, seed_table(0), g_level >= 0 ? seed_table(1) : nullptr, g_level, ego, nullptr, nullptr, st);
+  // SGL's three graphs differ: the two view chains sum into gd, then the main chain adds it and applies Adam
+  SRB_TRY(run_chain(s, w, &s->adj_view[0], seed_table(0), nullptr, -1, true, w.gd, nullptr, st));
+  SRB_TRY(run_chain(s, w, &s->adj_view[1], seed_table(1), nullptr, -1, true, w.gd, w.gd, st));
+  return run_chain(s, w, &s->adj, seed_table(2), nullptr, -1, true, nullptr, w.gd, st);
 }

@@ -91,7 +91,7 @@ struct SpmmArgs {
   float* Y;
   const float* extra;
   float extra_scale;
-  // optional backward seed table (engine.cu, run_chain_seeded): y += seed[row] where seed_mask has the row's bit; the
+  // optional backward seed table (engine.cu, run_chain): y += seed[row] where seed_mask has the row's bit; the
   // table holds nothing elsewhere
   const uint32_t* seed_mask;
   const float* seed;

@@ -585,32 +585,38 @@ def test_rank_hit_masks_and_fast_measure(torch_cuda, golden, tiny_triples, tiny_
     assert fast == slow
 
 
+def _norm_adj(pu, pi, U, I):
+    """D^-1/2 [[0, R], [R^T, 0]] D^-1/2 of the (user, item) pairs, as float32 CSR."""
+    n = U + I
+    half = sp.csr_matrix((np.ones(len(pu), np.float32), (pu, pi.astype(np.int64) + U)), shape=(n, n), dtype=np.float32)
+    adj = half + half.T
+    d = np.asarray(adj.sum(1)).ravel()
+    dinv = np.power(d, -0.5, out=np.zeros_like(d), where=d > 0).astype(np.float32)  # a dropped view may isolate a node
+    return sp.diags(dinv).dot(adj).dot(sp.diags(dinv)).tocsr().astype(np.float32)
+
+
 class _SynthData:
     """What TrainEngine reads from an Interaction, for a random bipartite graph."""
 
     def __init__(self, rng, U, I, n_pairs):
-        import scipy.sparse as sp_
         pu = rng.integers(0, U, n_pairs).astype(np.int32)
         pi = (rng.zipf(1.5, n_pairs) % I).astype(np.int32)
         pu[:U] = np.arange(U)  # every user and item appears
         pi[:I] = np.arange(I)
         self.user_num, self.item_num = U, I
         self.pair_users, self.pair_items = pu, pi
-        n = U + I
-        half = sp_.csr_matrix((np.ones(n_pairs, np.float32), (pu, pi.astype(np.int64) + U)), shape=(n, n), dtype=np.float32)
-        adj = half + half.T
-        d = np.asarray(adj.sum(1)).ravel()
-        dinv = np.where(d > 0, d ** -0.5, 0).astype(np.float32)
-        self.norm_adj = sp_.diags(dinv).dot(adj).dot(sp_.diags(dinv)).tocsr().astype(np.float32)
+        self.norm_adj = _norm_adj(pu, pi, U, I)
         self.training_data = []
 
 
 @pytest.mark.parametrize("name,d,L,lcl", [("XSimGCL", 32, 2, 1), ("XSimGCL", 128, 3, 3), ("XSimGCL", 64, 1, 1), ("XSimGCL", 64, 2, 0),
-                                          ("SimGCL", 128, 2, 0), ("LightGCN", 32, 3, 0), ("MF", 128, 0, 0)])
+                                          ("SimGCL", 128, 2, 0), ("SimGCL", 64, 1, 0), ("SimGCL", 32, 5, 0), ("SGL", 64, 1, 0),
+                                          ("SGL", 128, 3, 0), ("LightGCN", 32, 3, 0), ("MF", 128, 0, 0)])
 def test_engine_steps_vs_oracle_other_widths_and_partial_batches(torch_cuda, orc, name, d, L, lcl):
     """The fused step against the float64 oracle at embedding sizes 32 / 128 (CUDA-core InfoNCE, other SpMM
-    instantiations), with every position of the contrastive layer, a short last batch and an EMPTY batch
-    (which must leave parameters to Adam's zero-gradient update, exactly like the oracle)."""
+    instantiations), with every position of the contrastive layer, one and five SimGCL layers, SGL on two
+    edge-dropped view graphs, a short last batch and an EMPTY batch (which must leave parameters to Adam's
+    zero-gradient update, exactly like the oracle)."""
     torch = torch_cuda
     from selfrec_b200.engine import TrainEngine
     rng = np.random.default_rng(d * 10 + L)
@@ -621,7 +627,14 @@ def test_engine_steps_vs_oracle_other_widths_and_partial_batches(torch_cuda, orc
     kw = dict(eps=0.2, tau=0.2, cl_rate=0.3, layer_cl=lcl) if name in ("XSimGCL", "SimGCL") else {}
     if name in ("MF", "LightGCN"):
         kw["l2_div"] = float(B)
+    if name == "SGL":
+        kw = dict(tau=0.2, cl_rate=0.3)
     eng = TrainEngine(name, data, d, L, B, 1e-2, 1e-3, init_user=torch.from_numpy(E0[:U]), init_item=torch.from_numpy(E0[U:]), **kw)
+    view_csr = None
+    if name == "SGL":  # edge dropout at rate 0.1, re-normalised (SGL.py:27-29)
+        keep = [rng.random(len(data.pair_users)) >= 0.1 for _ in range(2)]
+        view_csr = [_norm_adj(data.pair_users[k], data.pair_items[k], U, I) for k in keep]
+        eng.set_view_graphs(*view_csr)
     views = 2 if name == "SimGCL" else 1
     p, m, v = E0.copy(), np.zeros_like(E0), np.zeros_like(E0)
     for step, b in enumerate((B, 17, 0, B), start=1):
@@ -638,7 +651,8 @@ def test_engine_steps_vs_oracle_other_widths_and_partial_batches(torch_cuda, orc
             g, ref = np.zeros((N, d)), None
         else:
             ref = orc.train_step(name, data.norm_adj if name != "MF" else None, p, U, u, i, j, n_layers=L, reg=1e-3,
-                                 batch_size=B, eps=0.2, tau=0.2, cl_rate=0.3, layer_cl=lcl, noise=None if noise is None else noise[:, :L])
+                                 batch_size=B, eps=0.2, tau=0.2, cl_rate=0.3, layer_cl=lcl, noise=None if noise is None else noise[:, :L],
+                                 view_csr=view_csr)
             g = ref["grad"]
         p, m, v = orc.adam_step(p, g.astype(np.float32), m, v, step, 1e-2)
         got = eng.params.cpu().numpy()
