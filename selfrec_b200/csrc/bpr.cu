@@ -180,10 +180,7 @@ __global__ void __launch_bounds__(256) scatter_add_rows_kernel(float* dst, const
   const int nn = sg.n_dev ? min(*sg.n_dev, sg.n) : sg.n;
   if (r >= nn) return;
   int row = sg.rows[r] + sg.row_off;
-  if (sg.row_hi > sg.row_lo) {  // sharded tables: only the rows this rank owns
-    if (row < sg.row_lo || row >= sg.row_hi) return;
-    row -= sg.row_lo;
-  } else if (sg.mod > 0) {  // cyclic ownership (bipartite sharding: user u lives on rank u % world, local row u / world)
+  if (sg.mod > 0) {  // cyclic ownership (bipartite sharding: user u lives on rank u % world, local row u / world)
     if (row % sg.mod != sg.rem) return;
     row /= sg.mod;
   }
@@ -339,7 +336,7 @@ extern "C" int srb_scatter_add_rows(float* dst, int32_t d, const float* src, con
   SRB_REQUIRE(n >= 0, "scatter: negative n");
   srb::ScatterSegs segs;
   segs.count = 1;
-  segs.s[0] = {src, rows, n_dev, n, row_off, scale, 0, 0};
+  segs.s[0] = {src, rows, n_dev, n, row_off, scale};
   return srb::scatter_segments(dst, d, segs, (cudaStream_t)stream);
 }
 
@@ -350,7 +347,7 @@ extern "C" int srb_scatter_add_segments(float* dst, int32_t d, int32_t n_segs, c
   segs.count = n_segs;
   for (int q = 0; q < n_segs; ++q) {
     SRB_REQUIRE(in[q].src && in[q].rows && in[q].n >= 0, "scatter: bad segment %d", q);
-    segs.s[q] = {in[q].src, in[q].rows, in[q].n_dev, in[q].n, in[q].row_off, in[q].scale, 0, 0};
+    segs.s[q] = {in[q].src, in[q].rows, in[q].n_dev, in[q].n, in[q].row_off, in[q].scale};
   }
   return srb::scatter_segments(dst, d, segs, (cudaStream_t)stream);
 }

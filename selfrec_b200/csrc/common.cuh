@@ -82,7 +82,6 @@ struct ScatterSeg {
   int32_t n;            // capacity / host count
   int32_t row_off;
   float scale;
-  int32_t row_lo, row_hi;  // optional filter (row_hi > row_lo): only rows[r] + row_off in [row_lo, row_hi), stored at - row_lo
   int32_t mod, rem;        // optional filter (mod > 0; cyclic row ownership): only rows with row % mod == rem, stored at row / mod
 };
 struct ScatterSegs {
@@ -90,6 +89,8 @@ struct ScatterSegs {
   ScatterSeg s[16];
 };
 int scatter_segments(float* dst, int d, const ScatterSegs& segs, cudaStream_t st);
+// a step's four losses (BPR, L2, cl_rate x the sum of n_nce InfoNCE losses, total) into out[4] (engine.cu)
+int finalize_losses(const float* bpr_losses, const float* nce_losses, int n_nce, float cl_rate, float* out, cudaStream_t st);
 
 // Adam step counter + bias corrections in double, like torch's Python floats (one thread)
 __device__ __forceinline__ void adam_prepare(int32_t* step, float* scalars, double lr, double b1, double b2) {

@@ -161,16 +161,11 @@ __global__ void build_cat_idx_kernel(const int32_t* batch, int cap, int n_users,
 }
 
 // rows of the [N, d] tables a batch touches: u, U + i, U + j, each listed ONCE (the bitmap de-duplicates: a hub user
-// sits in a batch many times) and classified by degree on the fly for the last-layer SpMM -- split rows (their
-// chunks go to hub_work), a CTA per long row, a warp per other row; the lane-group class stays empty -- into four
-// segments of capacity 3*cap; counters[c] ends up as the size of class c, counters[4] as the number of chunks.
-// counters[0..7] and row_mask are zeroed by step_begin_kernel.
-// With a row range [row_begin, row_begin + n_local) (row-sharded tables) only the rows of that range are listed,
-// as LOCAL row ids of the rank's CSR slice; the bitmap always covers all batch rows (global ids).
+// sits in a batch many times) and classified by degree for the last-layer SpMM into four segments of capacity 3*cap
+// (list_batch_row).  counters[0..7] and row_mask are zeroed by step_begin_kernel.
 __global__ void __launch_bounds__(256) build_batch_rows_kernel(const int32_t* batch, int cap, int n_users, const int32_t* rowptr,
-                                                               int row_begin, int n_local, int32_t* rows, int32_t* counters,
-                                                               uint32_t* row_mask, int32_t* hub_first, int32_t* hub_work,
-                                                               int hub_cap) {
+                                                               int32_t* rows, int32_t* counters, uint32_t* row_mask,
+                                                               int32_t* hub_first, int32_t* hub_work, int hub_cap) {
   const int t = blockIdx.x * blockDim.x + threadIdx.x;
   pdl_wait();
   pdl_trigger();
@@ -178,32 +173,10 @@ __global__ void __launch_bounds__(256) build_batch_rows_kernel(const int32_t* ba
   const int sec = t / cap, k = t % cap;
   if (sec >= 3 || k >= b) return;
   const int32_t* u = batch + SRB_BATCH_HEADER;
-  const int grow = (sec == 0) ? u[k] : n_users + u[sec * cap + k];
-  const uint32_t bit = 1u << (grow & 31);
-  if (atomicOr(row_mask + (grow >> 5), bit) & bit) return;  // listed already
-  const int row = grow - row_begin;
-  if (row < 0 || row >= n_local) return;
-  const int deg = rowptr[row + 1] - rowptr[row];
-  // only ~3B rows: parallelism is scarce, so no row shares a warp and rows above 4 warp-iterations get a CTA
-  const int cls = (hub_first && deg >= SRB_HUB_MIN_NNZ) ? 0 : (deg >= 128 ? 1 : 2);
-  // warp-aggregated slot allocation per class
-  const unsigned mine = __match_any_sync(__activemask(), cls);
-  const int lane = threadIdx.x & 31;
-  const int leader = __ffs(mine) - 1;
-  int base = 0;
-  if (lane == leader) base = atomicAdd(counters + cls, __popc(mine));
-  base = __shfl_sync(mine, base, leader);
-  const int slot = base + __popc(mine & ((1u << lane) - 1));
-  rows[cls * 3 * cap + slot] = row;
-  if (cls == 0) {
-    const int nch = (deg + SRB_HUB_CHUNK - 1) / SRB_HUB_CHUNK;
-    const int first = atomicAdd(counters + 4, nch);
-    hub_first[slot] = first;
-    for (int c = 0; c < nch && first + c < hub_cap; ++c) {
-      hub_work[2 * (first + c)] = row;
-      hub_work[2 * (first + c) + 1] = c;
-    }
-  }
+  const int row = (sec == 0) ? u[k] : n_users + u[sec * cap + k];
+  const uint32_t bit = 1u << (row & 31);
+  if (atomicOr(row_mask + (row >> 5), bit) & bit) return;  // listed already
+  list_batch_row(row, rowptr[row + 1] - rowptr[row], 0, rows, 3 * cap, counters, hub_first, hub_work, hub_cap);
 }
 
 // first kernel of a graph model's step: Adam's bias corrections, the batch-row counters + bitmap cleared, and the batch
@@ -236,6 +209,10 @@ __global__ void finalize_losses_kernel(const float* bpr_losses, const float* nce
   out[1] = bpr_losses[1];
   out[2] = cl;
   out[3] = bpr_losses[0] + bpr_losses[1] + cl;
+}
+
+int finalize_losses(const float* bpr_losses, const float* nce_losses, int n_nce, float cl_rate, float* out, cudaStream_t st) {
+  return launch_kernel(finalize_losses_kernel, 1, 1, 0, st, "finalize_losses_kernel", bpr_losses, nce_losses, n_nce, cl_rate, out);
 }
 
 static int spmm_simple(const srb_step_desc* s, const srb_graph_csr* g, const float* x, float* y, const float* extra,
@@ -329,7 +306,7 @@ static int run_chain(const srb_step_desc* s, const Ws& w, const srb_graph_csr* g
 }
 
 static ScatterSeg seg(const float* src, const int32_t* rows, const int32_t* n_dev, int n, int row_off, float scale) {
-  ScatterSeg g = {src, rows, n_dev, n, row_off, scale, 0, 0};
+  ScatterSeg g = {src, rows, n_dev, n, row_off, scale};
   return g;
 }
 
@@ -445,8 +422,8 @@ extern "C" int srb_train_step(const srb_step_desc* s, void* stream) {
     const int threads = std::max(n_words, 3 * B * (d / 4));
     SRB_TRY(launch_kernel(step_begin_kernel, (threads + 255) / 256, 256, 0, st, "step_begin_kernel", s->step_dev, s->scalars, s->lr,
                           s->beta1, s->beta2, w.n_hub, n_words, s->batch, B, U, N, d, w.seed, w.n_seed));
-    SRB_TRY(launch_kernel(build_batch_rows_kernel, (3 * B + 255) / 256, 256, 0, st, "build_batch_rows_kernel", s->batch, B, U, s->adj.rowptr, 0,
-                          U + s->n_items, w.batch_rows, w.n_hub, w.row_mask, w.hub_cap ? w.hub_first : nullptr, w.hub_work, w.hub_cap));
+    SRB_TRY(launch_kernel(build_batch_rows_kernel, (3 * B + 255) / 256, 256, 0, st, "build_batch_rows_kernel", s->batch, B, U, s->adj.rowptr,
+                          w.batch_rows, w.n_hub, w.row_mask, w.hub_cap ? w.hub_first : nullptr, w.hub_work, w.hub_cap));
   } else {
     SRB_TRY(srb_adam_prepare(s->step_dev, s->scalars, s->lr, s->beta1, s->beta2, stream));
   }
@@ -558,8 +535,7 @@ extern "C" int srb_train_step(const srb_step_desc* s, void* stream) {
     n_nce = 1;
   }
   if (fk) SRB_TRY(check_cuda(cudaStreamWaitEvent(st, fk->join, 0), "join wait"));
-  SRB_TRY(launch_kernel(finalize_losses_kernel, 1, 1, 0, st, "finalize_losses_kernel", w.bpr_losses, w.nce_losses, n_nce, s->cl_rate,
-                        s->losses));
+  SRB_TRY(finalize_losses(w.bpr_losses, w.nce_losses, n_nce, s->cl_rate, s->losses, st));
 
   // ---- backward + Adam ----
   const size_t plane = (size_t)B * d;

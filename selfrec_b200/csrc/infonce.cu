@@ -13,7 +13,6 @@
 //           dV1 += G V2 (registers, one atomic pass), dV2 += G^T V1 (red.v4 per tile)
 //                                                                            (6 n^2 d flop)
 //   finish  back through F.normalize, loss = mean(lse - S_ii)
-#include <stdlib.h>
 #include "common.cuh"
 #include "infonce_tc.cuh"
 
@@ -533,16 +532,6 @@ __global__ void __launch_bounds__(256) nce_tc_finish_kernel(const NceArgs a) {
   }
 }
 
-// 0 = auto (tensor cores when d == 64), 1 = CUDA-core tiles, 2 = tensor cores
-static int nce_impl() {
-  static int impl = -1;
-  if (impl < 0) {
-    const char* e = getenv("SRB_NCE_IMPL");
-    impl = e ? atoi(e) : 0;
-  }
-  return impl;
-}
-
 // tensor-core pipeline: prep (exact rows + TF32 hi/lo parts) -> pass A (LSE + view-1 gradient) -> pass B -> finish
 static int nce_launch_tc(const NceArgs& a, int n_problems, cudaStream_t st) {
   const int np = a.np;
@@ -712,10 +701,8 @@ extern "C" int srb_infonce_fwd_bwd(const srb_infonce_desc* d, void* stream) {
     p.loss_acc = p.lse + a.np;
   }
   cudaStream_t st = (cudaStream_t)stream;
-  const int impl = srb::nce_impl();
   // the tensor-core LSE pass shifts by the bound 1/tau of a cosine logit: needs exp(-2/tau) representable
-  if (d->d == 64 && d->b_cos && impl != 1 && d->n_problems <= 2 && a.inv_tau <= 40.f) return srb::nce_launch_tc(a, d->n_problems, st);
-  SRB_REQUIRE(impl != 2, "infonce: SRB_NCE_IMPL=2 (tensor cores) needs d == 64, b_cos and temperature >= 0.025");
+  if (d->d == 64 && d->b_cos && d->n_problems <= 2 && a.inv_tau <= 40.f) return srb::nce_launch_tc(a, d->n_problems, st);
   switch (d->d) {
     case 32: return srb::nce_launch<32>(a, d->n_problems, st);
     case 64: return srb::nce_launch<64>(a, d->n_problems, st);

@@ -105,32 +105,9 @@ __global__ void __launch_bounds__(256) shard_batch_rows_kernel(const BatchRowsAr
   const uint32_t bit = 1u << (row & 31);
   if (atomicOr((user ? a.umask : a.imask) + (row >> 5), bit) & bit) return;  // listed already
   const int32_t* rowptr = user ? a.ru_rowptr : a.rt_rowptr;
-  int32_t* rows = user ? a.rows_u : a.rows_i;
-  int32_t* counters = a.cnt + (user ? 0 : 8);
-  int32_t* hfirst = user ? a.hfirst_u : a.hfirst_i;
-  int32_t* hwork = user ? a.hwork_u : a.hwork_i;
-  const int hcap = user ? a.hcap_u : a.hcap_i;
-  const int capr = user ? a.cap : 2 * a.cap;
-  const int deg = rowptr[row + 1] - rowptr[row];
-  // few rows: parallelism is scarce, so no row shares a warp and rows above 4 warp-iterations get a CTA
-  const int cls = (hfirst && deg >= SRB_HUB_MIN_NNZ) ? 0 : (deg >= 128 ? 1 : 2);
-  const unsigned mine = __match_any_sync(__activemask(), cls + (user ? 0 : 4));
-  const int lane = threadIdx.x & 31;
-  const int leader = __ffs(mine) - 1;
-  int base = 0;
-  if (lane == leader) base = atomicAdd(counters + cls, __popc(mine));
-  base = __shfl_sync(mine, base, leader);
-  const int slot = base + __popc(mine & ((1u << lane) - 1));
-  rows[cls * capr + slot] = row;
-  if (cls == 0) {
-    const int nch = (deg + SRB_HUB_CHUNK - 1) / SRB_HUB_CHUNK;
-    const int first = atomicAdd(counters + 4, nch);
-    hfirst[slot] = first;
-    for (int q = 0; q < nch && first + q < hcap; ++q) {
-      hwork[2 * (first + q)] = row;
-      hwork[2 * (first + q) + 1] = q;
-    }
-  }
+  // a warp may list users and items at once: item keys are offset by 4 so that the two lists allocate slots apart
+  list_batch_row(row, rowptr[row + 1] - rowptr[row], user ? 0 : 4, user ? a.rows_u : a.rows_i, user ? a.cap : 2 * a.cap,
+                 a.cnt + (user ? 0 : 8), user ? a.hfirst_u : a.hfirst_i, user ? a.hwork_u : a.hwork_i, user ? a.hcap_u : a.hcap_i);
 }
 
 // compact table of the rows a batch reads: slot = section * cap + k (sections: u, i, j, unique u, unique i).
@@ -173,16 +150,6 @@ __global__ void __launch_bounds__(256) shard_gather_kernel(const GatherArgs a) {
 #pragma unroll 1
     for (int q = 0; q < a.n_dst; ++q) st4(a.dst[q] + (size_t)slot * D + c, v);
   }
-}
-
-__global__ void shard_finalize_losses_kernel(const float* bpr_losses, const float* nce_losses, int n_nce, float cl_rate, float* out) {
-  float cl = 0.f;
-  for (int q = 0; q < n_nce; ++q) cl += nce_losses[q];
-  cl *= cl_rate;
-  out[0] = bpr_losses[0];
-  out[1] = bpr_losses[1];
-  out[2] = cl;
-  out[3] = bpr_losses[0] + bpr_losses[1] + cl;
 }
 
 static int64_t al256(int64_t x) { return (x + 255) / 256 * 256; }
@@ -419,7 +386,6 @@ static void item_epilogue(const Ctx& c, const Epi& e, SpmmArgs& a) {
   const srb_shard_desc* s = c.s;
   epi_common(c, e, a);
   a.noise_row_base = c.U;
-  a.row_begin = 0;
   a.Y = e.y_i >= 0 ? c.mine(e.y_i) : nullptr;
   a.extra = e.extra_i;
   a.sum_in = e.sum_in_i;
@@ -509,7 +475,6 @@ static int layer(const Ctx& c, const float* xu, const float* xi, const Epi& e) {
     epi_common(c, e, a);
     a.noise_row_base = c.rank;  // global id of local user row r: rank + r * world
     a.noise_row_stride = c.G;
-    a.row_begin = 0;
     a.Y = e.y_u;
     a.extra = e.extra_u;
     a.sum_in = e.sum_in_u;
@@ -604,11 +569,11 @@ static int gather(const Ctx& c, const float* utab, const float* itab, int64_t ct
 }
 
 static ScatterSeg useg(const Ctx& c, const float* src, const int32_t* rows, const int32_t* n_dev, float scale) {
-  ScatterSeg g = {src, rows, n_dev, c.B, 0, scale, 0, 0, c.G, c.rank};
+  ScatterSeg g = {src, rows, n_dev, c.B, 0, scale, c.G, c.rank};
   return g;
 }
 static ScatterSeg iseg(const Ctx& c, const float* src, const int32_t* rows, const int32_t* n_dev, float scale) {
-  ScatterSeg g = {src, rows, n_dev, c.B, 0, scale, 0, 0};
+  ScatterSeg g = {src, rows, n_dev, c.B, 0, scale};
   return g;
 }
 
@@ -822,8 +787,7 @@ extern "C" int srb_shard_step(const srb_shard_desc* s, void* stream) {
     SRB_TRY(srb_infonce_fwd_bwd(&q, stream));
     n_nce = 2;
   }
-  shard_finalize_losses_kernel<<<1, 1, 0, st>>>(bpr_losses, nce_losses, n_nce, s->cl_rate, s->losses);
-  SRB_TRY(post_launch("shard_finalize_losses_kernel"));
+  SRB_TRY(finalize_losses(bpr_losses, nce_losses, n_nce, s->cl_rate, s->losses, st));
 
   // ---- Horner backward (engine.cu: one merged chain) + Adam ----
   const float cm = 1.f / (float)(lg ? L + 1 : L);

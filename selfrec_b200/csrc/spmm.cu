@@ -6,7 +6,6 @@
 //
 // HBM/L2-bound integer + fp32 work: no tensor cores here by design (see the kernel comment
 // for the lane mapping).
-#include <stdlib.h>
 #include "spmm_args.cuh"
 
 namespace srb {
@@ -42,15 +41,14 @@ __device__ __forceinline__ void spmm_epilogue(const SpmmArgs& a, int row, int gl
       st4(dst + HALF, acc1);
       return;
     }
-    const size_t off = (size_t)(a.row_begin + row) * D + gl * 4;
+    const size_t off = (size_t)row * D + gl * 4;
     float4 y0 = acc0, y1 = acc1;
     if (a.extra && valid) {
       y0 = f4_fma(a.extra_scale, *reinterpret_cast<const float4*>(a.extra + off), y0);
       y1 = f4_fma(a.extra_scale, *reinterpret_cast<const float4*>(a.extra + off + HALF), y1);
     }
     if (a.seed && valid) {
-      const int grow = a.row_begin + row;
-      if ((__ldg(a.seed_mask + (grow >> 5)) >> (grow & 31)) & 1u) {
+      if ((__ldg(a.seed_mask + (row >> 5)) >> (row & 31)) & 1u) {
         y0 = f4_add(y0, *reinterpret_cast<const float4*>(a.seed + off));
         y1 = f4_add(y1, *reinterpret_cast<const float4*>(a.seed + off + HALF));
       }
@@ -64,7 +62,7 @@ __device__ __forceinline__ void spmm_epilogue(const SpmmArgs& a, int row, int gl
         }
       } else {
         const uint32_t stp = a.pstep ? (uint32_t)*a.pstep : 0u;
-        const uint32_t grow = (uint32_t)(a.noise_row_base + (a.row_begin + row) * a.noise_row_stride);
+        const uint32_t grow = (uint32_t)(a.noise_row_base + row * a.noise_row_stride);
         // counter = (row, column block | view << 16, layer tag, step): (view, step) pairs never share a stream
         const uint32_t vw = a.poff.y << 16;
         const uint4 r0 = philox4x32_10(make_uint4(grow, (uint32_t)gl | vw, a.poff.x, stp), a.pkey);
@@ -161,24 +159,8 @@ __device__ __forceinline__ void spmm_epilogue(const SpmmArgs& a, int row, int gl
 // Each lane loads one (col, val) pair per iteration (coalesced, prefetched one iteration ahead) and
 // the pairs are walked with group-wide shuffles; every X-row gather is two 128-bit ld.global.nc per
 // lane (LPR lanes x 16 B = one contiguous half row), issued 2*SB at a time before the FMAs.
-//
-// ASYNC (tables beyond L2, D >= 64): the product is then bound by how many bytes of gathers an SM keeps in flight, and
-// the LDG path is capped by the registers that receive the data (8 x 16 B per lane, ~130 KB per SM at the occupancy
-// the kernel reaches).  Every second sub-batch is therefore fetched with cp.async into a per-lane staging slot in
-// shared memory (each lane reads back exactly the 2 x 16 B it requested: no cross-lane hand-off, only
-// cp.async.wait_group), issued BEFORE the register sub-batch: twice the bytes in flight with the same registers.
-__device__ __forceinline__ void cp_async16(void* smem_dst, const void* gsrc) {
-  const uint32_t s = (uint32_t)__cvta_generic_to_shared(smem_dst);
-  asm volatile("cp.async.ca.shared.global [%0], [%1], 16;" ::"r"(s), "l"(gsrc) : "memory");
-}
-__device__ __forceinline__ void cp_async_commit() { asm volatile("cp.async.commit_group;" ::: "memory"); }
-__device__ __forceinline__ void cp_async_wait_all() { asm volatile("cp.async.wait_group 0;" ::: "memory"); }
-
-constexpr int SPMM_STAGE_F4 = 8 * 32;  // float4 slots per warp: 4 rows x 2 halves x 32 lanes (4 KB)
-
-template <int D, bool MASKED, bool ASYNC = false>
-__device__ __forceinline__ void spmm_gather(const SpmmArgs& a, int p, int end, int stride, int gl, float4& acc0, float4& acc1,
-                                            float4* stg = nullptr) {
+template <int D, bool MASKED>
+__device__ __forceinline__ void spmm_gather(const SpmmArgs& a, int p, int end, int stride, int gl, float4& acc0, float4& acc1) {
   constexpr int LPR = D / 8;
   constexpr int HALF = D / 2;
   constexpr int SB = LPR < 4 ? LPR : 4;  // sub-batch: 2*SB independent 128-bit gathers per lane in flight
@@ -205,43 +187,7 @@ __device__ __forceinline__ void spmm_gather(const SpmmArgs& a, int p, int end, i
       vn = a.stream ? __ldcs(a.vals + p + stride + gl) : __ldg(a.vals + p + stride + gl);
       if (masked) hitn = (__ldg(a.col_mask + (cn >> 5)) >> (cn & 31)) & 1u;
     }
-    if (!masked && ASYNC && LPR >= 2 * SB) {
-#pragma unroll
-      for (int j0 = 0; j0 < LPR; j0 += 2 * SB) {
-        if (j0 > 0 && !__any_sync(SRB_FULL_MASK, p + j0 < end)) break;
-        float vb[SB];
-#pragma unroll
-        for (int j = 0; j < SB; ++j) {  // second sub-batch: shared-memory staging slots of this lane
-          const int cc = __shfl_sync(SRB_FULL_MASK, c, j0 + SB + j, LPR);
-          vb[j] = __shfl_sync(SRB_FULL_MASK, v, j0 + SB + j, LPR);
-          const float* xr = a.X + (size_t)cc * D + gl * 4;
-          cp_async16(stg + (2 * j) * 32, xr);
-          cp_async16(stg + (2 * j + 1) * 32, xr + HALF);
-        }
-        cp_async_commit();
-        float vv[SB];
-        float4 x0[SB], x1[SB];
-#pragma unroll
-        for (int j = 0; j < SB; ++j) {  // first sub-batch: registers
-          const int cc = __shfl_sync(SRB_FULL_MASK, c, j0 + j, LPR);
-          vv[j] = __shfl_sync(SRB_FULL_MASK, v, j0 + j, LPR);
-          const float* xr = a.X + (size_t)cc * D + gl * 4;
-          x0[j] = ldg4(xr);
-          x1[j] = ldg4(xr + HALF);
-        }
-#pragma unroll
-        for (int j = 0; j < SB; ++j) {
-          acc0 = f4_fma(vv[j], x0[j], acc0);
-          acc1 = f4_fma(vv[j], x1[j], acc1);
-        }
-        cp_async_wait_all();
-#pragma unroll
-        for (int j = 0; j < SB; ++j) {
-          acc0 = f4_fma(vb[j], stg[(2 * j) * 32], acc0);
-          acc1 = f4_fma(vb[j], stg[(2 * j + 1) * 32], acc1);
-        }
-      }
-    } else if (!masked) {
+    if (!masked) {
 #pragma unroll
       for (int j0 = 0; j0 < LPR; j0 += SB) {
         if (j0 > 0 && !__any_sync(SRB_FULL_MASK, p + j0 < end)) break;
@@ -312,13 +258,11 @@ __device__ __forceinline__ void xor_reduce_groups(float4& acc0, float4& acc1, in
 // A power-law graph at config-5 scale has rows with millions of non-zeros; one CTA walking such a row alone would
 // take longer than the rest of the product, so those rows are cut into chunks here and summed (in chunk order:
 // deterministic) by the main kernel.
-template <int D, bool MASKED, bool ASYNC>
+template <int D, bool MASKED>
 __global__ void __launch_bounds__(256) spmm_hub_kernel(const SpmmArgs a) {
   constexpr int LPR = D / 8;
   const int lane = threadIdx.x & 31;
   const int wib = threadIdx.x >> 5;
-  __shared__ float4 stage[ASYNC ? 8 * SPMM_STAGE_F4 : 1];
-  float4* stg = ASYNC ? stage + wib * SPMM_STAGE_F4 + lane : nullptr;
   const int grp = lane / LPR;
   const int gl = lane % LPR;
   pdl_wait();
@@ -344,7 +288,7 @@ __global__ void __launch_bounds__(256) spmm_hub_kernel(const SpmmArgs a) {
     const int wbeg = beg + wib * per;
     const int wend = min(end, wbeg + per);
     float4 acc0 = f4_zero(), acc1 = f4_zero();
-    spmm_gather<D, MASKED, ASYNC>(a, wbeg + grp * LPR, wend, 32, gl, acc0, acc1, stg);
+    spmm_gather<D, MASKED>(a, wbeg + grp * LPR, wend, 32, gl, acc0, acc1);
     xor_reduce_groups(acc0, acc1, LPR);
     if (grp == 0) {
       part[wib][0][gl] = acc0;
@@ -368,12 +312,10 @@ __global__ void __launch_bounds__(256) spmm_hub_kernel(const SpmmArgs a) {
 }
 
 // Short segments of the column-blocked lists: a warp each (lane groups stride the segment, like a "long" row).
-template <int D, bool MASKED, bool ASYNC>
+template <int D, bool MASKED>
 __global__ void __launch_bounds__(256) spmm_seg_warp_kernel(const SpmmArgs a) {
   constexpr int LPR = D / 8;
   const int lane = threadIdx.x & 31;
-  __shared__ float4 stage[ASYNC ? 8 * SPMM_STAGE_F4 : 1];
-  float4* stg = ASYNC ? stage + (threadIdx.x >> 5) * SPMM_STAGE_F4 + lane : nullptr;
   const int grp = lane / LPR;
   const int gl = lane % LPR;
   const int warp0 = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
@@ -384,7 +326,7 @@ __global__ void __launch_bounds__(256) spmm_seg_warp_kernel(const SpmmArgs a) {
     const int w = __ldg(a.order_warp + k);
     const int beg = __ldg(a.seg + 2 * w), end = __ldg(a.seg + 2 * w + 1);
     float4 acc0 = f4_zero(), acc1 = f4_zero();
-    spmm_gather<D, MASKED, ASYNC>(a, beg + grp * LPR, end, 32, gl, acc0, acc1, stg);
+    spmm_gather<D, MASKED>(a, beg + grp * LPR, end, 32, gl, acc0, acc1);
     xor_reduce_groups(acc0, acc1, LPR);
     if (grp == 0) {
       float* dst = a.hub_part + (size_t)w * D + gl * 4;
@@ -425,14 +367,12 @@ __global__ void __launch_bounds__(256) spmm_hub_finish_kernel(const SpmmArgs a) 
   }
 }
 
-template <int D, bool MASKED, bool ASYNC>
+template <int D, bool MASKED>
 __global__ void __launch_bounds__(256) spmm_csr_kernel(const SpmmArgs a) {
   constexpr int LPR = D / 8;     // lanes per row
   constexpr int RPW = 32 / LPR;  // rows per warp (short rows)
   const int lane = threadIdx.x & 31;
   const int wib = threadIdx.x >> 5;
-  __shared__ float4 stage[ASYNC ? 8 * SPMM_STAGE_F4 : 1];
-  float4* stg = ASYNC ? stage + wib * SPMM_STAGE_F4 + lane : nullptr;
   const int grp = lane / LPR;
   const int gl = lane % LPR;
   const int warp0 = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
@@ -465,7 +405,7 @@ __global__ void __launch_bounds__(256) spmm_csr_kernel(const SpmmArgs a) {
     const int wbeg = beg + wib * per;
     const int wend = min(end, wbeg + per);
     float4 acc0 = f4_zero(), acc1 = f4_zero();
-    spmm_gather<D, MASKED, ASYNC>(a, wbeg + grp * LPR, wend, 32, gl, acc0, acc1, stg);
+    spmm_gather<D, MASKED>(a, wbeg + grp * LPR, wend, 32, gl, acc0, acc1);
     xor_reduce_groups(acc0, acc1, LPR);
     if (grp == 0) {
       part[wib][0][gl] = acc0;
@@ -500,7 +440,7 @@ __global__ void __launch_bounds__(256) spmm_csr_kernel(const SpmmArgs a) {
     }
     if (is_long) p += grp * LPR;
     float4 acc0 = f4_zero(), acc1 = f4_zero();
-    spmm_gather<D, MASKED, ASYNC>(a, p, end, is_long ? 32 : LPR, gl, acc0, acc1, stg);
+    spmm_gather<D, MASKED>(a, p, end, is_long ? 32 : LPR, gl, acc0, acc1);
     if (is_long) {  // combine the lane groups; group 0 owns the row
       xor_reduce_groups(acc0, acc1, LPR);
       valid = valid && grp == 0;
@@ -659,25 +599,24 @@ int launch_reduce_rows(const SpmmArgs& a, const ReduceArgs& r, int d, cudaStream
   return post_launch("reduce_rows_kernel");
 }
 
-template <int D, bool M, bool AS>
+template <int D, bool M>
 static int launch_spmm_dma(const SpmmArgs& a, int hub_blocks, int blocks, cudaStream_t st) {
   if (hub_blocks > 0) {
     if (a.seg && a.n_warp > 0) {
       const int wb = max(1, min((a.n_warp + 7) / 8, blocks));
-      SRB_TRY(launch_kernel(spmm_seg_warp_kernel<D, M, AS>, wb, 256, 0, st, "spmm_seg_warp_kernel", a));
+      SRB_TRY(launch_kernel(spmm_seg_warp_kernel<D, M>, wb, 256, 0, st, "spmm_seg_warp_kernel", a));
     }
-    SRB_TRY(launch_kernel(spmm_hub_kernel<D, M, AS>, hub_blocks, 256, 0, st, "spmm_hub_kernel", a));
+    SRB_TRY(launch_kernel(spmm_hub_kernel<D, M>, hub_blocks, 256, 0, st, "spmm_hub_kernel", a));
     const int nh = a.n_vlong_dev ? a.n_rows : a.n_huge;  // (device-counted lists: the capacity)
     SRB_TRY(launch_kernel(spmm_hub_finish_kernel<D>, max(1, min((nh + 7) / 8, hub_blocks)), 256, 0, st, "spmm_hub_finish_kernel", a));
   }
-  return launch_kernel(spmm_csr_kernel<D, M, AS>, blocks, 256, 0, st, "spmm_csr_kernel", a);
+  return launch_kernel(spmm_csr_kernel<D, M>, blocks, 256, 0, st, "spmm_csr_kernel", a);
 }
 
 template <int D>
 static int launch_spmm_d(const SpmmArgs& a, int hub_blocks, int blocks, cudaStream_t st) {
-  if (a.col_mask != nullptr) return launch_spmm_dma<D, true, false>(a, hub_blocks, blocks, st);
-  if (D >= 64 && a.async_stage) return launch_spmm_dma<D, false, (D >= 64)>(a, hub_blocks, blocks, st);
-  return launch_spmm_dma<D, false, false>(a, hub_blocks, blocks, st);
+  if (a.col_mask != nullptr) return launch_spmm_dma<D, true>(a, hub_blocks, blocks, st);
+  return launch_spmm_dma<D, false>(a, hub_blocks, blocks, st);
 }
 
 int launch_spmm(const SpmmArgs& a, int d, cudaStream_t st) {
@@ -699,17 +638,6 @@ int launch_spmm(const SpmmArgs& a, int d, cudaStream_t st) {
     case 128: return launch_spmm_d<128>(a, (int)hub_blocks, (int)blocks, st);
     default: set_error("spmm: unsupported d=%d (32, 64, 128)", d); return SRB_ERR_ARG;
   }
-}
-
-// SRB_SPMM_ASYNC=1 stages every second gather sub-batch through cp.async + shared memory (measurement switch; results
-// are bit-identical).  Off by default: it doubles the bytes in flight, but every staged row pays an LDGSTS + LDS round
-// trip through the shared-memory port; run tools/config5_probe.py with and without it to compare.
-static bool async_stage_enabled() {
-  static const int on = [] {
-    const char* e = getenv("SRB_SPMM_ASYNC");
-    return (e && e[0] == '1') ? 1 : 0;
-  }();
-  return on != 0;
 }
 
 int fill_args(const srb_spmm_desc* d, SpmmArgs& a) {
@@ -773,14 +701,12 @@ int fill_args(const srb_spmm_desc* d, SpmmArgs& a) {
   a.w2 = (float)(1.0 - d->beta2);
   a.aeps = d->adam_eps;
   a.world = 0;
-  a.row_begin = 0;
   a.noise_row_base = 0;
   a.noise_row_stride = 1;
   a.peer_mc = 0;
   a.ps = PeerSync{};
   // (rows + columns) x d x 4 bytes of dense operands beyond 3/4 of the L2 (37.5 MB on an H100): stream the one-touch data
   a.stream = ((long long)d->n_rows + d->n_cols) * d->d * 4 > l2_bytes() / 4 * 3;
-  a.async_stage = a.stream && async_stage_enabled();  // (opt-in measurement switch, see async_stage_enabled)
   a.stage_rank = a.stage_cap = 0;
   for (int g = 0; g < 8; ++g) a.peer[g] = a.peer_sum[g] = a.peer_p[g] = a.stage_peer[g] = nullptr;
   for (int g = 0; g < 9; ++g) a.stage_bounds[g] = 0;

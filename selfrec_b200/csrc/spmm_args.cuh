@@ -111,14 +111,12 @@ struct SpmmArgs {
   const float* ascal;
   float b2, w1, w2, aeps;  // beta2, 1 - beta1, 1 - beta2 (rounded from double like torch's Python floats)
   int32_t world;
-  int32_t row_begin;  // global index of local row 0 (epilogue tensors are indexed by global row)
   float* peer[8];      // layer output -> every rank's buffer
   float* peer_sum[8];  // running sum  -> every rank's buffer
   float* peer_p[8];    // updated parameters (Adam epilogue) -> every rank's copy
   int32_t stream;          // tables larger than L2: CSR arrays and outputs are touched once per product -> evict-first accesses
-  int32_t async_stage;     // with `stream`: every second gather sub-batch goes through cp.async + shared memory (more bytes in flight)
   int32_t peer_mc;         // the one peer address is an NVSwitch multicast mapping: stores go out as multimem.st
-  int32_t noise_row_base;  // Philox row id = noise_row_base + (row_begin + row) * noise_row_stride: the GLOBAL id of a row of a
+  int32_t noise_row_base;  // Philox row id = noise_row_base + row * noise_row_stride: the GLOBAL id of a row of a
   int32_t noise_row_stride;  // sharded table (cyclic user blocks: base = rank, stride = world)
   // partial-sum push (bipartite sharding, item-side product): row r of this rank's partial product goes to the
   // staging area of the rank that owns item r: stage_peer[o] + ((size_t)stage_rank * stage_cap + r - stage_bounds[o]) * D
@@ -148,6 +146,34 @@ int launch_spmm(const SpmmArgs& a, int d, cudaStream_t st);
 int launch_reduce_rows(const SpmmArgs& a, const ReduceArgs& r, int d, cudaStream_t st);
 int launch_rows_epilogue(const SpmmArgs& a, int d, cudaStream_t st);  // Y[r] = epilogue(X[r]), r < n_rows
 int fill_args(const srb_spmm_desc* d, SpmmArgs& a);
+
+// Appends one batch row of degree deg to a device-classified row list of the last forward layer (the format of
+// srb_spmm_desc.n_vlong_dev): rows holds four segments of capacity cap -- split rows (only with hub_first; their
+// chunks go to hub_work), a CTA per row of >= 128 non-zeros, a warp per other row; the lane-group class stays empty.
+// A batch has only a few thousand rows, so parallelism is scarce and no row shares a warp.  counters[c] counts class c,
+// counters[4] the chunks.  Slots are allocated per warp among the threads with the same class + key_off, so lists
+// filled by one warp take different key offsets.
+__device__ __forceinline__ void list_batch_row(int row, int deg, int key_off, int32_t* rows, int cap, int32_t* counters,
+                                               int32_t* hub_first, int32_t* hub_work, int hub_cap) {
+  const int cls = (hub_first && deg >= SRB_HUB_MIN_NNZ) ? 0 : (deg >= 128 ? 1 : 2);
+  const unsigned mine = __match_any_sync(__activemask(), cls + key_off);
+  const int lane = threadIdx.x & 31;
+  const int leader = __ffs(mine) - 1;
+  int base = 0;
+  if (lane == leader) base = atomicAdd(counters + cls, __popc(mine));
+  base = __shfl_sync(mine, base, leader);
+  const int slot = base + __popc(mine & ((1u << lane) - 1));
+  rows[cls * cap + slot] = row;
+  if (cls == 0) {
+    const int nch = (deg + SRB_HUB_CHUNK - 1) / SRB_HUB_CHUNK;
+    const int first = atomicAdd(counters + 4, nch);
+    hub_first[slot] = first;
+    for (int c = 0; c < nch && first + c < hub_cap; ++c) {
+      hub_work[2 * (first + c)] = row;
+      hub_work[2 * (first + c) + 1] = c;
+    }
+  }
+}
 
 
 

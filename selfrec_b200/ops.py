@@ -5,7 +5,6 @@ computation is a hand-written sm_90a kernel reached through ctypes with raw poin
 All ops are stream-ordered on torch's current stream and raise SrbError without a GPU.
 """
 import ctypes as C
-import os
 
 import numpy as np
 import torch
@@ -245,9 +244,7 @@ class SparseAdj:
         if self.n_huge:
             ent = self._hub_part.get(d)
             if ent is None:
-                segs = None
-                if os.environ.get("SRB_HUB_COLBLOCK", "1") != "0":
-                    segs = column_blocked_segments(self.rowptr, self.colidx, self.row_order[: self.n_huge].to(torch.int64), self.shape[1], d)
+                segs = column_blocked_segments(self.rowptr, self.colidx, self.row_order[: self.n_huge].to(torch.int64), self.shape[1], d)
                 n_part = segs["n_seg"] if segs else self.n_work
                 ent = self._hub_part[d] = (torch.empty((n_part, d), device=self.device, dtype=torch.float32), segs)
             part, segs = ent
