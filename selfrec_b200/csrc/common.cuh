@@ -89,6 +89,22 @@ struct ScatterSegs {
   ScatterSeg s[16];
 };
 int scatter_segments(float* dst, int d, const ScatterSegs& segs, cudaStream_t st);
+
+// The backward seed tables of a graph model's step (engine.cu, both training steps).  LightGCN, XSimGCL: F and G;
+// SimGCL: F; SGL: F of the encoders on adj_view[0], adj_view[1], adj.  SeedRows places them in a step's layout.
+struct SeedRows {
+  int32_t user_off[3], item_off[3];  // row of user / item 0 in table t (ScatterSeg.row_off)
+  int32_t user_mod, user_rem;        // cyclic user ownership (ScatterSeg.mod / rem), or 0
+};
+struct SeedGrads {  // a batch's compact loss gradients, [cap, d] per batch list
+  const int32_t* batch;              // SRB_BATCH_HEADER counts, then the lists u | i | j | unique u | unique i
+  int cap, d;
+  const float *emb, *l2;             // BPR and LightGCN's L2 term on E0: [3][cap, d] at u, i, j
+  const float *nce_u[2], *nce_i[2];  // InfoNCE views 1, 2 at the unique users / items (SGL: nce_u at cat)
+  const int32_t *cat, *n_cat;        // SGL: table rows of the unique users, then of the unique items
+};
+// Which gradient enters which table, with what scale (one scatter); returns the level where G enters, or -1 (run_chain)
+int seed_segments(int model, int n_layers, int layer_cl, const SeedGrads& g, const SeedRows& r, ScatterSegs& segs);
 // a step's four losses (BPR, L2, cl_rate x the sum of n_nce InfoNCE losses, total) into out[4] (engine.cu)
 int finalize_losses(const float* bpr_losses, const float* nce_losses, int n_nce, float cl_rate, float* out, cudaStream_t st);
 

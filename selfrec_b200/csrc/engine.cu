@@ -215,6 +215,57 @@ int finalize_losses(const float* bpr_losses, const float* nce_losses, int n_nce,
   return launch_kernel(finalize_losses_kernel, 1, 1, 0, st, "finalize_losses_kernel", bpr_losses, nce_losses, n_nce, cl_rate, out);
 }
 
+int seed_segments(int model, int n_layers, int layer_cl, const SeedGrads& g, const SeedRows& r, ScatterSegs& segs) {
+  const int B = g.cap, L = n_layers;
+  const size_t plane = (size_t)B * g.d;
+  const int32_t* rows = g.batch + SRB_BATCH_HEADER;  // u | i | j | unique u | unique i
+  const int32_t* n_dev = g.batch;                    // b, unique users, unique items
+  const float cm = 1.f / (float)((model == SRB_MODEL_LIGHTGCN || model == SRB_MODEL_SGL) ? L + 1 : L);
+  segs.count = 0;
+  auto add = [&](int t, bool item, const float* src, const int32_t* idx, const int32_t* n, int cap, float scale) {
+    segs.s[segs.count++] = {src, idx, n, cap, item ? r.item_off[t] : r.user_off[t], scale, item ? 0 : r.user_mod, item ? 0 : r.user_rem};
+  };
+  auto add_bpr = [&](int t, const float* src, float scale) {  // rows u, i, j
+    add(t, false, src, rows, n_dev, B, scale);
+    add(t, true, src + plane, rows + B, n_dev, B, scale);
+    add(t, true, src + 2 * plane, rows + 2 * B, n_dev, B, scale);
+  };
+  auto add_nce = [&](int t, int view, float scale) {  // unique batch users, unique items
+    add(t, false, g.nce_u[view], rows + 3 * B, n_dev + 1, B, scale);
+    add(t, true, g.nce_i[view], rows + 4 * B, n_dev + 2, B, scale);
+  };
+  int g_level = -1;
+  switch (model) {
+    case SRB_MODEL_LIGHTGCN:  // the L2 term regularises the raw E0: G = F + its gradient at the ego level
+      add_bpr(0, g.emb, cm);
+      add_bpr(1, g.emb, cm);
+      add_bpr(1, g.l2, 1.f);
+      g_level = 0;
+      break;
+    case SRB_MODEL_XSIMGCL:
+      // view 1 = final (mean) rows, view 2 = layer l* output (XSimGCL.py:45-50); G = view 2's gradient, plus F unless
+      // l* is the ego layer, which the mean leaves out
+      g_level = (layer_cl >= 1 && layer_cl <= L) ? layer_cl : 0;
+      for (int t = 0; t < (g_level ? 2 : 1); ++t) {
+        add_bpr(t, g.emb, cm);
+        add_nce(t, 0, cm);
+      }
+      add_nce(1, 1, 1.f);
+      break;
+    case SRB_MODEL_SIMGCL:  // all three encoders are the same linear map of E0: one merged chain
+      add_bpr(0, g.emb, cm);
+      add_nce(0, 0, cm);
+      add_nce(0, 1, cm);
+      break;
+    case SRB_MODEL_SGL:  // cat holds table rows already: the user offset applies
+      add(0, false, g.nce_u[0], g.cat, g.n_cat, 2 * B, cm);
+      add(1, false, g.nce_u[1], g.cat, g.n_cat, 2 * B, cm);
+      add_bpr(2, g.emb, cm);
+      break;
+  }
+  return g_level;
+}
+
 static int spmm_simple(const srb_step_desc* s, const srb_graph_csr* g, const float* x, float* y, const float* extra,
                        bool adam, cudaStream_t st, const uint32_t* col_mask = nullptr, const float* seed = nullptr,
                        const uint32_t* seed_mask = nullptr) {
@@ -551,55 +602,15 @@ extern "C" int srb_train_step(const srb_step_desc* s, void* stream) {
     return srb_adam_step(s->params, s->adam_m, s->adam_v, w.acc0, (int64_t)N * d, s->scalars, s->beta1, s->beta2, s->adam_eps,
                          stream);
   }
-  const bool ego = s->model == SRB_MODEL_LIGHTGCN || s->model == SRB_MODEL_SGL;
-  const float cm = 1.f / (float)(ego ? L + 1 : L);
-  // one scatter fills every seed table: table t's rows are shifted by t * N
   auto seed_table = [&](int t) { return w.seed + (size_t)t * N * d; };
+  const SeedGrads gr = {s->batch, B, d, w.g_emb, w.g_l2, {g1a, g2a}, {g1b, g2b}, w.idx_cat, w.n_cat};
+  const SeedRows rows = {{0, N, 2 * N}, {U, N + U, 2 * N + U}, 0, 0};  // seed table t: rows t * N + [0, N)
   ScatterSegs sg = {};
-  auto add = [&](int t, const float* src, const int32_t* rows, const int32_t* n_dev, int n, int row_off, float scale) {
-    sg.s[sg.count++] = seg(src, rows, n_dev, n, t * N + row_off, scale);
-  };
-  auto add_bpr = [&](int t, const float* g, float scale) {  // rows u, U + i, U + j
-    add(t, g, u_idx, b_dev, B, 0, scale);
-    add(t, g + plane, i_idx, b_dev, B, U, scale);
-    add(t, g + 2 * plane, j_idx, b_dev, B, U, scale);
-  };
-  auto add_nce = [&](int t, const float* gu, const float* gi, float scale) {  // unique batch users, U + unique items
-    add(t, gu, uq_u, nu_dev, B, 0, scale);
-    add(t, gi, uq_i, ni_dev, B, U, scale);
-  };
-  int g_level = -1;  // LightGCN, XSimGCL: the level where table 1 (G) enters instead of F
-  switch (s->model) {
-    case SRB_MODEL_LIGHTGCN:  // the L2 term regularises the raw E0: G = F + its gradient at the ego level
-      add_bpr(0, w.g_emb, cm);
-      add_bpr(1, w.g_emb, cm);
-      add_bpr(1, w.g_l2, 1.f);
-      g_level = 0;
-      break;
-    case SRB_MODEL_XSIMGCL:
-      // view 1 = final (mean) rows, view 2 = layer l* output (XSimGCL.py:45-50); G = view 2's gradient, plus F unless
-      // l* is the ego layer, which the mean leaves out
-      g_level = (s->layer_cl >= 1 && s->layer_cl <= L) ? s->layer_cl : 0;
-      for (int t = 0; t < (g_level ? 2 : 1); ++t) {
-        add_bpr(t, w.g_emb, cm);
-        add_nce(t, g1a, g1b, cm);
-      }
-      add_nce(1, g2a, g2b, 1.f);
-      break;
-    case SRB_MODEL_SIMGCL:  // all three encoders are the same linear map of E0: one merged chain
-      add_bpr(0, w.g_emb, cm);
-      add_nce(0, g1a, g1b, cm);
-      add_nce(0, g2a, g2b, cm);
-      break;
-    case SRB_MODEL_SGL:  // a table per encoder graph: adj_view[0], adj_view[1], adj
-      add(0, g1a, w.idx_cat, w.n_cat, 2 * B, 0, cm);
-      add(1, g2a, w.idx_cat, w.n_cat, 2 * B, 0, cm);
-      add_bpr(2, w.g_emb, cm);
-      break;
-  }
+  const int g_level = seed_segments(s->model, L, s->layer_cl, gr, rows, sg);
   SRB_TRY(scatter_segments(w.seed, d, sg, st));
   if (s->model != SRB_MODEL_SGL)
-    return run_chain(s, w, &s->adj, seed_table(0), g_level >= 0 ? seed_table(1) : nullptr, g_level, ego, nullptr, nullptr, st);
+    return run_chain(s, w, &s->adj, seed_table(0), g_level >= 0 ? seed_table(1) : nullptr, g_level, s->model == SRB_MODEL_LIGHTGCN,
+                     nullptr, nullptr, st);
   // SGL's three graphs differ: the two view chains sum into gd, then the main chain adds it and applies Adam
   SRB_TRY(run_chain(s, w, &s->adj_view[0], seed_table(0), nullptr, -1, true, w.gd, nullptr, st));
   SRB_TRY(run_chain(s, w, &s->adj_view[1], seed_table(1), nullptr, -1, true, w.gd, w.gd, st));

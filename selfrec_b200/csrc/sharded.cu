@@ -20,9 +20,9 @@
 //
 // Batch losses: the <= 5B rows a batch reads are pushed by their owners into a compact [5B, d] table on every
 // rank (sections u, i, j, unique u, unique i), BPR / InfoNCE run replicated on it with the single-GPU kernels,
-// and the compact gradients are scattered into the owners' accumulators (user rows) or every replica (item
-// rows).  Persistent state (parameters, Adam moments) has exactly one writer per row, so the replicas of the item
-// table are bit-identical on all ranks by construction.
+// and the compact gradients are scattered once into engine.cu's backward seed tables (user rows on their owner, item
+// rows on every rank), whose chain runs on layer().  Persistent state (parameters, Adam moments) has exactly one writer
+// per row, so the replicas of the item table are bit-identical on all ranks by construction.
 //
 // Replaces the same reference code as engine.cu (the batch-loop bodies of LightGCN.py:21-29, SimGCL.py:25-36,
 // XSimGCL.py:27-37); world == 1 runs the same sequence without staging or barriers.
@@ -64,13 +64,30 @@ __global__ void shard_barrier_kernel(const BarrierArgs b) {
   }
 }
 
+// First kernel of the step (engine.cu's step_begin_kernel on this layout): Adam's bias corrections, n_words words cleared,
+// and the batch rows u, i, j of the first n_seed seed slots cleared where the seed scatter puts them, a float4 per thread.
+__global__ void __launch_bounds__(256) shard_begin_kernel(int32_t* step, float* scalars, double lr, double b1, double b2, int32_t* words,
+                                                          int n_words, const int32_t* batch, int cap, int d, float* seed, int n_seed,
+                                                          const SeedRows r) {
+  const int t = blockIdx.x * blockDim.x + threadIdx.x;
+  if (t == 0) adam_prepare(step, scalars, lr, b1, b2);
+  if (t < n_words) words[t] = 0;
+  const int k0 = t / (d / 4), c = (t % (d / 4)) * 4;
+  const int sec = k0 / cap, k = k0 % cap;
+  if (sec >= 3 || k >= min(batch[0], cap)) return;
+  const int id = batch[SRB_BATCH_HEADER + sec * cap + k];
+  if (sec == 0 && id % r.user_mod != r.user_rem) return;  // another rank's user
+  for (int q = 0; q < n_seed; ++q)
+    st4(seed + (size_t)(sec == 0 ? (id + r.user_off[q]) / r.user_mod : id + r.item_off[q]) * d + c, f4_zero());
+}
+
 // Bits of the batch's (local) users / items (masks of the row-sparse first backward product: umask over this rank's
 // local user rows, imask over all items), and -- from the thread that sets
 // a bit first, so every row is listed once -- the batch's rows of this rank's two blocks, classified by degree for the
 // last forward layer (nothing but the batch rows of the final mean is read): local users -> rows of Ru, items ->
 // rows of Rt.  Lists follow srb_spmm_desc.n_vlong_dev: four segments (split, CTA, warp, lane group -- unused) of
 // capacity cap (users) / 2 * cap (items); cnt[0..3] class sizes and cnt[4] chunks of the user list, cnt[8..] of the
-// item list.  cnt and both bitmaps are zeroed by the caller.
+// item list.  cnt and both bitmaps are zeroed by shard_begin_kernel.
 struct BatchRowsArgs {
   const int32_t* batch;
   int cap;
@@ -191,8 +208,9 @@ static SymPlan sym_plan(int64_t I, int64_t d, int64_t B, int world) {
 
 struct LocalPlan {
   int64_t ctrl;  // [0] barrier epoch, [1] error flag (zeroed once by the host, never by a step)
-  int64_t xu[2], su, clu, v2u, au[2], gdu;
-  int64_t v2_i, gdi;
+  int64_t xu[2], su, clu, v2u, au[2];
+  int64_t seed;  // backward seed slots, [2][Ug, d] (this rank's users) then [2][I, d] (the complete item replica)
+  int64_t v2_i;
   int64_t g_emb, g_l2, g_nce, bpr_scratch, bpr_losses, nce_losses, ar, umask, imask, cnt, nce_ws, total;
   int64_t rows_u, rows_i, hfirst_u, hfirst_i, hwork_u, hwork_i;  // batch-row lists of the last forward layer
   int64_t nce_ws_bytes;
@@ -215,9 +233,8 @@ static LocalPlan local_plan(int64_t I, int64_t Ug, int64_t d, int64_t B, int64_t
   p.v2u = take(und);
   p.au[0] = take(und);
   p.au[1] = take(und);
-  p.gdu = take(und);
+  p.seed = take(2 * und + 2 * ind);  // contiguous: one scatter fills all four slots
   p.v2_i = take(ind);
-  p.gdi = take(ind);
   p.g_emb = take(3 * B * d * 4);
   p.g_l2 = take(3 * B * d * 4);
   p.g_nce = take(4 * B * d * 4);
@@ -225,7 +242,7 @@ static LocalPlan local_plan(int64_t I, int64_t Ug, int64_t d, int64_t B, int64_t
   p.bpr_losses = take(2 * 4);
   p.nce_losses = take(4 * 4);
   p.ar = take(2 * B * 4);
-  // one memset clears both bitmaps and the list counters
+  // shard_begin_kernel clears both bitmaps and the list counters: [umask, nce_ws)
   p.umask = take(((Ug + 31) / 32) * 4 + 4);  // bitmap over this rank's local user rows
   p.imask = take(((I + 31) / 32) * 4);
   p.cnt = take(16 * 4);
@@ -252,6 +269,8 @@ struct Ctx {
   float* symf(int64_t off, int q) const { return (float*)((char*)s->sym[q] + off); }
   float* mine(int64_t off) const { return (float*)(sym + off); }
   float* lw(int64_t off) const { return (float*)(loc + off); }
+  float* seed_u(int t) const { return lw(lp.seed) + (size_t)t * Ug * d; }
+  float* seed_i(int t) const { return lw(lp.seed) + ((size_t)2 * Ug + (size_t)t * I) * d; }
 };
 
 // SRB_SHARD_SYNC=barrier: separate barrier launches between the kernels of a layer instead of waits / signals folded
@@ -322,8 +341,8 @@ struct Epi {
   float* sum_out_i = nullptr;
   int64_t sum_push_i = -1;     // symmetric offset: the item running sum also goes to every rank (clean forward for eval)
   float sum_scale = 1.f;
-  const float* extra_u = nullptr;
-  const float* extra_i = nullptr;
+  const float* seed_u = nullptr;     // backward seed slot added at the batch rows (umask / imask), or null
+  const float* seed_i = nullptr;
   bool adam = false;
   const uint32_t* mask_u = nullptr;  // bitmap over this rank's users (columns of Rt)
   const uint32_t* mask_i = nullptr;  // bitmap over items (columns of Ru)
@@ -387,7 +406,8 @@ static void item_epilogue(const Ctx& c, const Epi& e, SpmmArgs& a) {
   epi_common(c, e, a);
   a.noise_row_base = c.U;
   a.Y = e.y_i >= 0 ? c.mine(e.y_i) : nullptr;
-  a.extra = e.extra_i;
+  a.seed = e.seed_i;  // (world > 1: added by the owner's reduction only, after the rank-ordered sum)
+  a.seed_mask = (const uint32_t*)(c.loc + c.lp.imask);
   a.sum_in = e.sum_in_i;
   a.sum_out = e.sum_out_i;
   if (e.adam) {
@@ -476,7 +496,8 @@ static int layer(const Ctx& c, const float* xu, const float* xi, const Epi& e) {
     a.noise_row_base = c.rank;  // global id of local user row r: rank + r * world
     a.noise_row_stride = c.G;
     a.Y = e.y_u;
-    a.extra = e.extra_u;
+    a.seed = e.seed_u;
+    a.seed_mask = (const uint32_t*)(c.loc + c.lp.umask);
     a.sum_in = e.sum_in_u;
     a.sum_out = e.sum_out_u;
     if (e.adam) {
@@ -568,15 +589,6 @@ static int gather(const Ctx& c, const float* utab, const float* itab, int64_t ct
   return post_launch("shard_gather_kernel");
 }
 
-static ScatterSeg useg(const Ctx& c, const float* src, const int32_t* rows, const int32_t* n_dev, float scale) {
-  ScatterSeg g = {src, rows, n_dev, c.B, 0, scale, c.G, c.rank};
-  return g;
-}
-static ScatterSeg iseg(const Ctx& c, const float* src, const int32_t* rows, const int32_t* n_dev, float scale) {
-  ScatterSeg g = {src, rows, n_dev, c.B, 0, scale};
-  return g;
-}
-
 static int make_ctx(const srb_shard_desc* s, void* stream, Ctx& c) {
   SRB_REQUIRE(s != nullptr, "shard: null desc");
   SRB_REQUIRE(s->model == SRB_MODEL_LIGHTGCN || s->model == SRB_MODEL_SIMGCL || s->model == SRB_MODEL_XSIMGCL,
@@ -637,19 +649,18 @@ extern "C" int srb_shard_step(const srb_shard_desc* s, void* stream) {
   cudaStream_t st = c.st;
   const int B = c.B, d = c.d, L = c.L;
   const int32_t* hdr = s->batch;
-  const int32_t* u_idx = s->batch + SRB_BATCH_HEADER;
-  const int32_t* i_idx = u_idx + B;
-  const int32_t* j_idx = i_idx + B;
-  const int32_t* uq_u = j_idx + B;
-  const int32_t* uq_i = uq_u + B;
   const int32_t *b_dev = hdr, *nu_dev = hdr + 1, *ni_dev = hdr + 2;
   const bool xs = s->model == SRB_MODEL_XSIMGCL, sg = s->model == SRB_MODEL_SIMGCL, lg = s->model == SRB_MODEL_LIGHTGCN;
   SRB_REQUIRE(lg || s->noise_mode == 2, "shard: SimGCL / XSimGCL need noise_mode 2");
 
-  SRB_TRY(srb_adam_prepare(s->step_dev, s->scalars, s->lr, s->beta1, s->beta2, stream));
   uint32_t* umask = (uint32_t*)(c.loc + c.lp.umask);
   uint32_t* imask = (uint32_t*)(c.loc + c.lp.imask);
-  SRB_TRY(check_cuda(cudaMemsetAsync(umask, 0, (size_t)(c.lp.nce_ws - c.lp.umask), st), "shard mask memset"));
+  // seed slot t: user u at row u / world + t * Ug, item i at 2 * Ug + t * I + i; SimGCL's slot 1 holds a forward buffer
+  const SeedRows rows = {{0, c.G * c.Ug}, {2 * c.Ug, 2 * c.Ug + c.I}, c.G, c.rank};
+  const int n_words = (int)((c.lp.nce_ws - c.lp.umask) / 4), threads = n_words > 3 * B * (d / 4) ? n_words : 3 * B * (d / 4);
+  shard_begin_kernel<<<(threads + 255) / 256, 256, 0, st>>>(s->step_dev, s->scalars, s->lr, s->beta1, s->beta2, (int32_t*)umask, n_words,
+                                                            s->batch, B, d, c.lw(c.lp.seed), sg ? 1 : 2, rows);
+  SRB_TRY(post_launch("shard_begin_kernel"));
   {
     BatchRowsArgs br = {};
     br.batch = s->batch;
@@ -690,8 +701,8 @@ extern "C" int srb_shard_step(const srb_shard_desc* s, void* stream) {
     // item table on every rank (the Philox stream is keyed by global row id: all replicas agree)
     float* zu = c.lw(c.lp.au[0]);
     float* zi = c.mine(c.sp.ai[0]);
-    float* x1u[2] = {c.lw(c.lp.au[1]), c.lw(c.lp.gdu)};
-    float* x1i[2] = {c.mine(c.sp.ai[1]), c.lw(c.lp.gdi)};
+    float* x1u[2] = {c.lw(c.lp.au[1]), c.seed_u(1)};
+    float* x1i[2] = {c.mine(c.sp.ai[1]), c.seed_i(1)};
     {
       Epi e;
       e.y_u = zu;
@@ -789,78 +800,38 @@ extern "C" int srb_shard_step(const srb_shard_desc* s, void* stream) {
   }
   SRB_TRY(finalize_losses(bpr_losses, nce_losses, n_nce, s->cl_rate, s->losses, st));
 
-  // ---- Horner backward (engine.cu: one merged chain) + Adam ----
-  const float cm = 1.f / (float)(lg ? L + 1 : L);
-  ScatterSegs fu = {}, fi = {}, cu = {}, ci = {}, eu = {}, ei = {};
-  fu.s[fu.count++] = useg(c, g_emb, u_idx, b_dev, cm);
-  fi.s[fi.count++] = iseg(c, g_emb + plane, i_idx, b_dev, cm);
-  fi.s[fi.count++] = iseg(c, g_emb + 2 * plane, j_idx, b_dev, cm);
-  int lcl = 0;
-  if (lg) {
-    eu.s[eu.count++] = useg(c, g_l2, u_idx, b_dev, 1.f);
-    ei.s[ei.count++] = iseg(c, g_l2 + plane, i_idx, b_dev, 1.f);
-    ei.s[ei.count++] = iseg(c, g_l2 + 2 * plane, j_idx, b_dev, 1.f);
-  } else if (xs) {
-    fu.s[fu.count++] = useg(c, g1a, uq_u, nu_dev, cm);
-    fi.s[fi.count++] = iseg(c, g1b, uq_i, ni_dev, cm);
-    ScatterSegs& tu = cl_hit ? cu : eu;
-    ScatterSegs& ti = cl_hit ? ci : ei;
-    tu.s[tu.count++] = useg(c, g2a, uq_u, nu_dev, 1.f);
-    ti.s[ti.count++] = iseg(c, g2b, uq_i, ni_dev, 1.f);
-    lcl = cl_hit ? s->layer_cl : 0;
-  } else {
-    fu.s[fu.count++] = useg(c, g1a, uq_u, nu_dev, cm);
-    fu.s[fu.count++] = useg(c, g2a, uq_u, nu_dev, cm);
-    fi.s[fi.count++] = iseg(c, g1b, uq_i, ni_dev, cm);
-    fi.s[fi.count++] = iseg(c, g2b, uq_i, ni_dev, cm);
-  }
-  auto merged = [](const ScatterSegs& a, const ScatterSegs* b) {
-    ScatterSegs m = a;
-    if (b)
-      for (int q = 0; q < b->count && m.count < 8; ++q) m.s[m.count++] = b->s[q];
-    return m;
-  };
-  const size_t ubytes = (size_t)c.Ug * d * 4, ibytes = (size_t)c.I * d * 4;
-  int x = 0;
+  // ---- backward: engine.cu's Horner chain (run_chain) on layer() + Adam ----
+  // Seed slots F (0) and G (1): slot g_level == k at level k.  Every rank reads only its own complete item slots, so the
+  // chain needs no synchronisation beyond layer()'s: the owner's reduction adds the item seed after the rank-ordered sum.
+  const SeedGrads gr = {s->batch, B, d, g_emb, g_l2, {g1a, g2a}, {g1b, g2b}, nullptr, nullptr};
+  ScatterSegs segs = {};
+  const int g_level = seed_segments(s->model, L, s->layer_cl, gr, rows, segs);
+  SRB_TRY(scatter_segments(c.lw(c.lp.seed), d, segs, st));
   float* au[2] = {c.lw(c.lp.au[0]), c.lw(c.lp.au[1])};
-  if (ubytes) SRB_TRY(check_cuda(cudaMemsetAsync(au[0], 0, ubytes, st), "shard memset"));
-  SRB_TRY(check_cuda(cudaMemsetAsync(c.mine(c.sp.ai[0]), 0, ibytes, st), "shard memset"));
-  if (c.Ug) SRB_TRY(scatter_segments(au[0], d, merged(fu, lcl == L ? &cu : nullptr), st));
-  SRB_TRY(scatter_segments(c.mine(c.sp.ai[0]), d, merged(fi, lcl == L ? &ci : nullptr), st));
-  // every rank's replica of the seed is complete before a peer's reduction may overwrite the other buffer: the
-  // ping-pong below only ever writes the buffer nobody reads in the same layer
-  for (int k = L - 1; k >= 1; --k) {
+  const float *xu = c.seed_u(g_level == L), *xi = c.seed_i(g_level == L);
+  for (int k = L - 1, x = 0; k >= 1; --k, x ^= 1) {
     Epi e;
-    e.y_u = au[x ^ 1];
-    e.y_i = c.sp.ai[x ^ 1];
-    if (k == L - 1) {  // the seed is non-zero at the batch rows only
+    e.y_u = au[x];
+    e.y_i = c.sp.ai[x];
+    e.seed_u = c.seed_u(g_level == k);
+    e.seed_i = c.seed_i(g_level == k);
+    if (k == L - 1) {  // the input is a seed slot: valid at the batch rows only
       e.mask_u = umask;
       e.mask_i = imask;
     }
-    SRB_TRY(layer(c, au[x], c.mine(c.sp.ai[x]), e));
-    x ^= 1;
-    SRB_TRY(wait_peers(c));  // the peers' reductions have stored their slices into this rank's copy: now add to it
-    if (c.Ug) SRB_TRY(scatter_segments(au[x], d, merged(fu, lcl == k ? &cu : nullptr), st));
-    SRB_TRY(scatter_segments(c.mine(c.sp.ai[x]), d, merged(fi, lcl == k ? &ci : nullptr), st));
-  }
-  const bool ego_add = lg || eu.count || ei.count;
-  float* gdu = c.lw(c.lp.gdu);
-  float* gdi = c.lw(c.lp.gdi);
-  if (ego_add) {
-    if (ubytes) SRB_TRY(check_cuda(cudaMemsetAsync(gdu, 0, ubytes, st), "shard memset"));
-    SRB_TRY(check_cuda(cudaMemsetAsync(gdi, 0, ibytes, st), "shard memset"));
-    if (c.Ug) SRB_TRY(scatter_segments(gdu, d, lg ? merged(fu, &eu) : eu, st));
-    SRB_TRY(scatter_segments(gdi, d, lg ? merged(fi, &ei) : ei, st));
+    SRB_TRY(layer(c, xu, xi, e));
+    xu = au[x];
+    xi = c.mine(c.sp.ai[x]);
   }
   Epi e;
   e.adam = true;
-  e.extra_u = ego_add ? gdu : nullptr;
-  e.extra_i = ego_add ? gdi : nullptr;
+  e.seed_u = g_level == 0 ? c.seed_u(1) : nullptr;  // the ego level takes G only (LightGCN's G holds F too)
+  e.seed_i = g_level == 0 ? c.seed_i(1) : nullptr;
   if (L == 1) {
     e.mask_u = umask;
     e.mask_i = imask;
   }
-  return layer(c, au[x], c.mine(c.sp.ai[x]), e);
+  return layer(c, xu, xi, e);
 }
 
 /* Clean forward for evaluation / save() (XSimGCL.py:40-41, 53-55): the final mean of this rank's users goes to

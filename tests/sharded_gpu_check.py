@@ -31,7 +31,13 @@ def main():
     cases = [("XSimGCL", 64, 3, dict(eps=0.2, tau=0.2, cl_rate=0.2, layer_cl=1)),
              ("XSimGCL", 64, 2, dict(eps=0.2, tau=0.2, cl_rate=0.2, layer_cl=2)),
              ("SimGCL", 128, 2, dict(eps=0.1, tau=0.2, cl_rate=0.5)),
-             ("LightGCN", 64, 3, dict(l2_div=512.0))]
+             ("LightGCN", 64, 3, dict(l2_div=512.0)),
+             # where the backward's second seed table G enters: XSimGCL at L = 1 gathers it in the only product, which
+             # also applies Adam; LightGCN at L = 1 adds it at the ego level of that product; XSimGCL with layer_cl = 0
+             # holds only view 2's gradient in G and adds it at the ego level
+             ("XSimGCL", 64, 1, dict(eps=0.2, tau=0.2, cl_rate=0.2, layer_cl=1)),
+             ("LightGCN", 64, 1, dict(l2_div=512.0)),
+             ("XSimGCL", 64, 3, dict(eps=0.2, tau=0.2, cl_rate=0.2, layer_cl=0))]
     graphs = {"powerlaw": synth.make_interaction((3000, 4000, 60000), seed=3),
               "zipf-split-rows": synth.make_device_interaction((30000, 8000, 1200000), seed=2, alpha=1.1)}
     # P2P stores | multicast stores | + in-switch reduce-scatter (the optional NVLS route, exercised at 2 ranks)

@@ -121,8 +121,8 @@ def test_bipartite_sharded_propagation_world2_gloo():
 def test_sharded_simgcl_step_algebra_model():
     """float64 model of what csrc/sharded.cu computes for one SimGCL step on G ranks -- cyclic users, replicated items,
     item rows as rank-ordered sums of partial products, ONE shared first product + per-view noise (SimGCL.py:85-88), the
-    last forward layer evaluated on the batch rows only, one merged backward chain whose first product is masked by the
-    batch rows -- against the oracle's plain restatement of SimGCL.py:25-36 (three full encoders, three backward chains).
+    last forward layer evaluated on the batch rows only, one merged backward chain on a seed table that holds the loss
+    gradients at the batch rows (the first product masked by them, the seed added after every later product) -- against the oracle's plain restatement of SimGCL.py:25-36 (three full encoders, three backward chains).
     Losses and the E0 gradient must agree to float64 rounding: the rewrites are algebra, not approximations."""
     sys.path.insert(0, os.path.join(ROOT, "oracle"))
     import oracle
