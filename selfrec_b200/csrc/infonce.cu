@@ -186,8 +186,12 @@ __global__ void __launch_bounds__(256) nce_prep_tc_kernel(const NceArgs a) {
     if (lane == 0) {
       p.inv1[i] = i1;
       p.inv2[i] = i2;
-      p.diag[i] = s12 * a.inv_tau;
-      p.part_l[i] = 0.f;  // softmax denominator l_i, accumulated by pass A
+      const float dg = s12 * a.inv_tau;
+      p.diag[i] = dg;
+      // softmax denominator l_i: its diagonal term from the exact S_ii here (the tensor-core S_ii is low by the
+      // accumulator's truncation, ~2^-21 of a unit cosine, and at small tau this term is nearly all of l_i); pass A
+      // adds the off-diagonal terms
+      p.part_l[i] = expf(dg - a.inv_tau);
     }
   }
   __syncthreads();

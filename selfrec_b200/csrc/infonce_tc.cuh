@@ -3,7 +3,8 @@
 // Same contract as infonce.cu (util/loss_torch.py:35-50 + autograd backward); the n x n logit matrix
 // lives only in registers.  Per problem, with V1, V2 the L2-normalised gathered views:
 //   pass A  rows = view-1 rows i:  E = exp(S - 1/tau)  (|S| <= 1/tau: cosines, so the shift needs no running max);
-//           l_i += sum_j E_ij (the softmax denominator) and, unnormalised, dV1_i += sum_{j != i} E_ij V2_j
+//           l_i += sum_{j != i} E_ij (the softmax denominator; prep seeds it with exp(S_ii - 1/tau) from the exact
+//           S_ii) and, unnormalised, dV1_i += sum_{j != i} E_ij V2_j
 //           -- forward (LSE) and the view-1 gradient in ONE sweep: the 1/l_i factor is applied afterwards
 //   pass B  rows = view-2 rows j:  G' = exp(S^T - lse_i) * w/(n tau), i != j;  dV2 += G' V1   (needs every l_i)
 //   finish  scales dV1 by w/(n tau l_i), adds the diagonal term (P_ii - 1) w/(n tau) v_i in exact fp32, then the
@@ -58,7 +59,7 @@ struct NtProblem {
   const int32_t* n_dev;
   float weight;
   const float* diag;     // [NP] exact S_ii
-  float* lsum;           // [NP] softmax denominators l_i = sum_j exp(S_ij - 1/tau) (zeroed by prep, accumulated by pass A)
+  float* lsum;           // [NP] softmax denominators l_i = sum_j exp(S_ij - 1/tau) (diagonal term by prep, the rest by pass A)
   float* dV1;            // [NP][64] accumulators (zeroed by prep)
   float* dV2;
   float* loss_acc;
@@ -219,11 +220,11 @@ __global__ void __launch_bounds__(NT_THREADS, 1) nce_tc_kernel(const __grid_cons
       const int rh = (j >> 1) & 1;                     // row_a or row_a + 8
       const float off = (MODE == 1) ? -sc : cc[cl];    // pass B: -inf for columns >= n
       float x = ex2_approx(fmaf(sv[j], sc, off));
+      x = (cb + cl == row_a + 8 * rh) ? 0.f : x;
       if (MODE == 1) {
         x = (cb + cl < n) ? x : 0.f;
-        l_run[rh] += x;  // the denominator includes the diagonal
+        l_run[rh] += x;  // off-diagonal terms only: prep seeded l_i with the exact diagonal term
       }
-      x = (cb + cl == row_a + 8 * rh) ? 0.f : x;
       const float h = to_tf32_rna(x);
       hi[j] = __float_as_uint(h);
       lo[j] = __float_as_uint(x - h);

@@ -430,26 +430,37 @@ def l2_reg_loss(reg, *args):
     return _L2Fn.apply(reg, *args)
 
 
-def infonce_raw(problems, d, temperature, b_cos=True, max_n=None):
-    """Run srb_infonce_fwd_bwd.  problems: list of dicts(table1, table2, idx, n, weight,
-    row_off1, row_off2).  Returns (losses [P], [(g1, g2)])."""
+def infonce_raw(problems, d, temperature, b_cos=True, max_n=None, workspace=None):
+    """Run srb_infonce_fwd_bwd.  problems: list of dicts(table1, table2, idx, n, and optionally n_dev,
+    weight, row_off1, row_off2, scale1, scale2, and g1 / g2 output tensors to write into).
+    workspace: optional uint8 device tensor to use instead of a fresh one (its whole size is offered).
+    Returns (losses [P], [(g1, g2)])."""
     lib = _lib.require_device()
     dev = problems[0]["table1"].device
     npb = len(problems)
-    mx = max(p["n"] for p in problems) if max_n is None else max_n
-    ws_bytes = lib.srb_infonce_workspace_bytes(mx, d, npb)
-    ws = torch.empty(max(ws_bytes, 16), device=dev, dtype=torch.uint8)
+    if not 1 <= npb <= 4:  # srb_infonce_desc.prob[4]
+        raise SrbError(f"infonce: n_problems must be 1..4 (got {npb})")
+    if workspace is None:
+        mx = max(p["n"] for p in problems) if max_n is None else max_n
+        ws_bytes = lib.srb_infonce_workspace_bytes(mx, d, npb)
+        ws = torch.empty(max(ws_bytes, 16), device=dev, dtype=torch.uint8)
+    else:
+        ws = workspace
+        ws_bytes = ws.numel() * ws.element_size()
     losses = torch.empty(npb, device=dev, dtype=torch.float32)
     desc = _lib.InfoNceDesc()
     desc.n_problems, desc.d, desc.b_cos, desc.temperature = npb, d, int(bool(b_cos)), float(temperature)
     outs = []
     for q, p in enumerate(problems):
-        g1 = torch.empty((p["n"], d), device=dev, dtype=torch.float32)
-        g2 = torch.empty((p["n"], d), device=dev, dtype=torch.float32)
+        g1 = p["g1"] if "g1" in p else torch.empty((p["n"], d), device=dev, dtype=torch.float32)
+        g2 = p["g2"] if "g2" in p else torch.empty((p["n"], d), device=dev, dtype=torch.float32)
+        for g in (g1, g2):
+            if g.shape != (p["n"], d) or g.dtype != torch.float32 or not g.is_contiguous():
+                raise SrbError(f"infonce: g1 / g2 of problem {q} must be contiguous float32 [{p['n']}, {d}]")
         pr = desc.prob[q]
         pr.table1, pr.table2 = _p(p["table1"]), _p(p["table2"])
         pr.row_off1, pr.row_off2 = p.get("row_off1", 0), p.get("row_off2", 0)
-        pr.scale1, pr.scale2 = 1.0, 1.0
+        pr.scale1, pr.scale2 = float(p.get("scale1", 1.0)), float(p.get("scale2", 1.0))
         pr.idx, pr.n_dev, pr.n, pr.weight = _p(p["idx"]), _p(p.get("n_dev")), p["n"], float(p.get("weight", 1.0))
         pr.g1, pr.g2 = _p(g1), _p(g2)
         pr.loss = C.c_void_p(losses.data_ptr() + 4 * q)
