@@ -560,8 +560,10 @@ int srb_sampler_ring_stop(srb_sampler* s);
  *   sym[q]   base of rank q's symmetric region (torch.distributed._symmetric_memory), sym_bytes each, zero-filled
  *            once before the first step; item parameters live at srb_shard_layout.item_params inside it
  *   workspace local, zero-filled once before the first step (it holds the barrier epoch)
- * Models: LightGCN, SimGCL, XSimGCL (same arithmetic as srb_train_step; noise from the in-kernel Philox stream,
- * keyed by GLOBAL row id, so a sharded run draws the noise the single-GPU engine draws).  world == 1 is valid.
+ * Models: LightGCN, SimGCL, XSimGCL, SGL (same arithmetic as srb_train_step; noise from the in-kernel Philox stream,
+ * keyed by GLOBAL row id, so a sharded run draws the noise the single-GPU engine draws).  SGL also propagates over the
+ * epoch's two view graphs, given as this rank's blocks of each (Ru_view / Rt_view, same layout as Ru / Rt; their split-row
+ * chunk counts must not exceed those of Ru / Rt, which size the plan).  world == 1 is valid.
  * ------------------------------------------------------------------------------------- */
 typedef struct srb_shard_desc {
   int32_t model;
@@ -595,6 +597,8 @@ typedef struct srb_shard_desc {
   void* fork_event;
   void* join_event;
   int32_t nvls; /* != 0 (needs sym_mc): reduce-scatter through the NVSwitch (multimem.ld_reduce) instead of P2P partial pushes */
+  srb_graph_csr Ru_view[2]; /* SGL: this rank's blocks of the epoch's two dropped, re-normalised graphs (else unused) */
+  srb_graph_csr Rt_view[2];
 } srb_shard_desc;
 
 typedef struct srb_shard_layout {
@@ -605,10 +609,12 @@ typedef struct srb_shard_layout {
   int64_t ctrl;            /* byte offset inside the workspace of int32 {barrier epoch, peer-timeout flag} */
 } srb_shard_layout;
 
-/* hub_chunks_u / hub_chunks_t: Ru.hub.n_work / Rt.hub.n_work of the rank's blocks (capacity of the per-batch split-row
+/* model: SRB_MODEL_* of the step (SGL needs more workspace: a third seed table per side, the batch-row lists of its views
+ * and a larger InfoNCE workspace; the other three share one layout).
+ * hub_chunks_u / hub_chunks_t: Ru.hub.n_work / Rt.hub.n_work of the rank's blocks (capacity of the per-batch split-row
  * lists of the last forward layer, which is evaluated on the batch rows only) */
-int srb_shard_plan(int32_t n_users, int32_t n_items, int32_t n_local_users, int32_t d, int32_t batch_cap,
-                     int32_t world, int32_t hub_chunks_u, int32_t hub_chunks_t, srb_shard_layout* out);
+int srb_shard_plan(int32_t model, int32_t n_users, int32_t n_items, int32_t n_local_users, int32_t d, int32_t batch_cap,
+                   int32_t world, int32_t hub_chunks_u, int32_t hub_chunks_t, srb_shard_layout* out);
 int srb_shard_step(const srb_shard_desc* desc, void* stream);
 /* clean forward (evaluation / save(), XSimGCL.py:40-41,53-55): out_user [n_local_users, d]; the complete item half
  * lands in every rank's symmetric region at item_final */

@@ -129,7 +129,7 @@ class ShardDesc(C.Structure):
         ("Ru", GraphCsr), ("Rt", GraphCsr), ("batch", VP), ("pu", VP), ("mu", VP), ("vu", VP), ("mi", VP), ("vi", VP),
         ("step_dev", VP), ("scalars", VP), ("losses", VP), ("sym", VP * 8), ("sym_mc", VP), ("sym_bytes", C.c_int64),
         ("workspace", VP), ("workspace_bytes", C.c_int64), ("fork_stream", VP), ("fork_event", VP), ("join_event", VP),
-        ("nvls", C.c_int32),
+        ("nvls", C.c_int32), ("Ru_view", GraphCsr * 2), ("Rt_view", GraphCsr * 2),
     ]
 
 
@@ -190,7 +190,8 @@ SYMBOLS = {
     "srb_sampler_ring_start": (C.c_int, [VP, C.c_int32, C.c_int32, C.c_int32]),
     "srb_sampler_ring_pop": (C.c_int, [VP, c_i32p]),
     "srb_sampler_ring_stop": (C.c_int, [VP]),
-    "srb_shard_plan": (C.c_int, [C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.POINTER(ShardLayout)]),
+    "srb_shard_plan": (C.c_int, [C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32,
+                                 C.POINTER(ShardLayout)]),
     "srb_shard_step": (C.c_int, [C.POINTER(ShardDesc), VP]),
     "srb_shard_forward": (C.c_int, [C.POINTER(ShardDesc), VP, VP]),
 }

@@ -170,7 +170,8 @@ __global__ void __launch_bounds__(256) bpr_grad_kernel(const BprArgs a) {
   }
 }
 
-template <int D>
+// SPLIT: some segment lists users and items together (ScatterSeg.item_min); without it the kernel is the plain scatter
+template <int D, bool SPLIT>
 __global__ void __launch_bounds__(256) scatter_add_rows_kernel(float* dst, const ScatterSegs segs) {
   const ScatterSeg& sg = segs.s[blockIdx.y];
   const int lane = threadIdx.x & 31;
@@ -179,10 +180,15 @@ __global__ void __launch_bounds__(256) scatter_add_rows_kernel(float* dst, const
   pdl_trigger();
   const int nn = sg.n_dev ? min(*sg.n_dev, sg.n) : sg.n;
   if (r >= nn) return;
-  int row = sg.rows[r] + sg.row_off;
-  if (sg.mod > 0) {  // cyclic ownership (bipartite sharding: user u lives on rank u % world, local row u / world)
-    if (row % sg.mod != sg.rem) return;
-    row /= sg.mod;
+  int row = sg.rows[r];
+  if (SPLIT && sg.item_min > 0 && row >= sg.item_min) {
+    row += sg.item_off - sg.item_min;  // an item row of a mixed user / item list: every rank keeps the complete item table
+  } else {
+    row += sg.row_off;
+    if (sg.mod > 0) {  // cyclic ownership (bipartite sharding: user u lives on rank u % world, local row u / world)
+      if (row % sg.mod != sg.rem) return;
+      row /= sg.mod;
+    }
   }
   for (int c = lane * 4; c < D; c += 128) {
     const float4 v = f4_scale(sg.scale, ldg4(sg.src + (size_t)r * D + c));
@@ -195,13 +201,19 @@ int scatter_segments(float* dst, int d, const ScatterSegs& segs, cudaStream_t st
   int max_n = 0;
   for (int q = 0; q < segs.count; ++q) max_n = segs.s[q].n > max_n ? segs.s[q].n : max_n;
   if (max_n == 0) return SRB_OK;
+  bool split = false;
+  for (int q = 0; q < segs.count; ++q) split = split || segs.s[q].item_min > 0;
   dim3 grid((max_n + 7) / 8, segs.count);
+#define SRB_SCATTER(D)                                                                                                            \
+  return split ? launch_kernel(scatter_add_rows_kernel<D, true>, grid, 256, 0, st, "scatter_add_rows_kernel", dst, segs)        \
+               : launch_kernel(scatter_add_rows_kernel<D, false>, grid, 256, 0, st, "scatter_add_rows_kernel", dst, segs);
   switch (d) {
-    case 32: return launch_kernel(scatter_add_rows_kernel<32>, grid, 256, 0, st, "scatter_add_rows_kernel", dst, segs);
-    case 64: return launch_kernel(scatter_add_rows_kernel<64>, grid, 256, 0, st, "scatter_add_rows_kernel", dst, segs);
-    case 128: return launch_kernel(scatter_add_rows_kernel<128>, grid, 256, 0, st, "scatter_add_rows_kernel", dst, segs);
+    case 32: SRB_SCATTER(32)
+    case 64: SRB_SCATTER(64)
+    case 128: SRB_SCATTER(128)
     default: set_error("scatter: unsupported d=%d (32, 64, 128)", d); return SRB_ERR_ARG;
   }
+#undef SRB_SCATTER
 }
 
 // Standalone l2_reg_loss (util/loss_torch.py:18-22) for the op-level drop-in, where the

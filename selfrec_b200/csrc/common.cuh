@@ -83,6 +83,8 @@ struct ScatterSeg {
   int32_t row_off;
   float scale;
   int32_t mod, rem;        // optional filter (mod > 0; cyclic row ownership): only rows with row % mod == rem, stored at row / mod
+  int32_t item_min;        // optional (> 0): rows[r] >= item_min are items, stored at rows[r] - item_min + item_off, unfiltered
+  int32_t item_off;
 };
 struct ScatterSegs {
   int count;
@@ -95,6 +97,8 @@ int scatter_segments(float* dst, int d, const ScatterSegs& segs, cudaStream_t st
 struct SeedRows {
   int32_t user_off[3], item_off[3];  // row of user / item 0 in table t (ScatterSeg.row_off)
   int32_t user_mod, user_rem;        // cyclic user ownership (ScatterSeg.mod / rem), or 0
+  int32_t item_min;                  // > 0: SGL's cat rows from item_min on are items (ScatterSeg.item_min), placed at
+                                     // item_off[t]; 0: cat rows are table rows of one [N, d] table per t
 };
 struct SeedGrads {  // a batch's compact loss gradients, [cap, d] per batch list
   const int32_t* batch;              // SRB_BATCH_HEADER counts, then the lists u | i | j | unique u | unique i

@@ -257,9 +257,12 @@ int seed_segments(int model, int n_layers, int layer_cl, const SeedGrads& g, con
       add_nce(0, 0, cm);
       add_nce(0, 1, cm);
       break;
-    case SRB_MODEL_SGL:  // cat holds table rows already: the user offset applies
-      add(0, false, g.nce_u[0], g.cat, g.n_cat, 2 * B, cm);
-      add(1, false, g.nce_u[1], g.cat, g.n_cat, 2 * B, cm);
+    case SRB_MODEL_SGL:  // cat holds users u and items U + i: one table row each (item_min 0), or split at item_min
+      for (int t = 0; t < 2; ++t) {
+        add(t, false, g.nce_u[t], g.cat, g.n_cat, 2 * B, cm);
+        segs.s[segs.count - 1].item_min = r.item_min;
+        segs.s[segs.count - 1].item_off = r.item_min > 0 ? r.item_off[t] : 0;
+      }
       add_bpr(2, g.emb, cm);
       break;
   }

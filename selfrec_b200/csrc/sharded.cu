@@ -24,8 +24,11 @@
 // rows on every rank), whose chain runs on layer().  Persistent state (parameters, Adam moments) has exactly one writer
 // per row, so the replicas of the item table are bit-identical on all ranks by construction.
 //
+// SGL propagates over three graphs: the normalised adjacency and the epoch's two dropped views, each given as this rank's
+// Ru / Rt blocks (srb_shard_desc.Ru_view / Rt_view).  Every layer() takes the block pair it runs on; the exchange is the same.
+//
 // Replaces the same reference code as engine.cu (the batch-loop bodies of LightGCN.py:21-29, SimGCL.py:25-36,
-// XSimGCL.py:27-37); world == 1 runs the same sequence without staging or barriers.
+// XSimGCL.py:27-37, SGL.py:30-41); world == 1 runs the same sequence without staging or barriers.
 #include <stdlib.h>
 #include "spmm_args.cuh"
 
@@ -88,12 +91,8 @@ __global__ void __launch_bounds__(256) shard_begin_kernel(int32_t* step, float* 
 // rows of Rt.  Lists follow srb_spmm_desc.n_vlong_dev: four segments (split, CTA, warp, lane group -- unused) of
 // capacity cap (users) / 2 * cap (items); cnt[0..3] class sizes and cnt[4] chunks of the user list, cnt[8..] of the
 // item list.  cnt and both bitmaps are zeroed by shard_begin_kernel.
-struct BatchRowsArgs {
-  const int32_t* batch;
-  int cap;
-  uint32_t* umask;
-  uint32_t* imask;
-  int world, rank;   // user u lives on rank u % world as local row u / world
+// SGL's three graphs share the batch rows and the bitmaps but not the degrees: the same thread lists the row for each.
+struct BatchRowLists {  // one graph's lists
   const int32_t* ru_rowptr;
   const int32_t* rt_rowptr;
   int32_t* rows_u;    // [4][cap]
@@ -105,6 +104,15 @@ struct BatchRowsArgs {
   int32_t* hfirst_i;  // [2 * cap] or null
   int32_t* hwork_i;
   int hcap_i;
+};
+struct BatchRowsArgs {
+  const int32_t* batch;
+  int cap;
+  uint32_t* umask;
+  uint32_t* imask;
+  int world, rank;   // user u lives on rank u % world as local row u / world
+  int n_graphs;      // 1, or SGL's 3 (the graph, view 1, view 2)
+  BatchRowLists g[3];
 };
 
 __global__ void __launch_bounds__(256) shard_batch_rows_kernel(const BatchRowsArgs a) {
@@ -121,10 +129,13 @@ __global__ void __launch_bounds__(256) shard_batch_rows_kernel(const BatchRowsAr
   }
   const uint32_t bit = 1u << (row & 31);
   if (atomicOr((user ? a.umask : a.imask) + (row >> 5), bit) & bit) return;  // listed already
-  const int32_t* rowptr = user ? a.ru_rowptr : a.rt_rowptr;
-  // a warp may list users and items at once: item keys are offset by 4 so that the two lists allocate slots apart
-  list_batch_row(row, rowptr[row + 1] - rowptr[row], user ? 0 : 4, user ? a.rows_u : a.rows_i, user ? a.cap : 2 * a.cap,
-                 a.cnt + (user ? 0 : 8), user ? a.hfirst_u : a.hfirst_i, user ? a.hwork_u : a.hwork_i, user ? a.hcap_u : a.hcap_i);
+  for (int q = 0; q < a.n_graphs; ++q) {
+    const BatchRowLists& l = a.g[q];
+    const int32_t* rowptr = user ? l.ru_rowptr : l.rt_rowptr;
+    // a warp may list users and items at once: item keys are offset by 4 so that the two lists allocate slots apart
+    list_batch_row(row, rowptr[row + 1] - rowptr[row], user ? 0 : 4, user ? l.rows_u : l.rows_i, user ? a.cap : 2 * a.cap,
+                   l.cnt + (user ? 0 : 8), user ? l.hfirst_u : l.hfirst_i, user ? l.hwork_u : l.hwork_i, user ? l.hcap_u : l.hcap_i);
+  }
 }
 
 // compact table of the rows a batch reads: slot = section * cap + k (sections: u, i, j, unique u, unique i).
@@ -139,6 +150,12 @@ struct GatherArgs {
   float* dst[8];
   int n_dst;
   int32_t* ar;  // [2*cap]: k and cap + k (index lists of the compact tables), written by block 0
+  // SGL (written by block 0 when cat is set): the unique users, then the unique items (SGL.py:120-121) as compact
+  // slots 3 cap + k / 4 cap + k (cat) and as table rows u / n_users + i (cat_id); n_cat = their count
+  int32_t* cat;
+  int32_t* cat_id;
+  int32_t* n_cat;
+  int n_users;
 };
 
 template <int D>
@@ -147,6 +164,15 @@ __global__ void __launch_bounds__(256) shard_gather_kernel(const GatherArgs a) {
   const int w = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
   if (a.ar && blockIdx.x == 0)
     for (int t = threadIdx.x; t < 2 * a.cap; t += blockDim.x) a.ar[t] = t;
+  if (a.cat && blockIdx.x == 0) {
+    const int nu = min(a.batch[1], a.cap), ni = min(a.batch[2], a.cap);
+    const int32_t* uq = a.batch + SRB_BATCH_HEADER + 3 * a.cap;  // unique users, then (at + cap) unique items
+    for (int t = threadIdx.x; t < nu + ni; t += blockDim.x) {
+      a.cat[t] = t < nu ? 3 * a.cap + t : 4 * a.cap + t - nu;
+      a.cat_id[t] = t < nu ? uq[t] : a.n_users + uq[a.cap + t - nu];
+    }
+    if (threadIdx.x == 0) *a.n_cat = nu + ni;
+  }
   const int slot = a.sec_lo * a.cap + w;
   if (slot >= a.sec_hi * a.cap) return;
   const int sec = slot / a.cap, k = slot % a.cap;
@@ -209,14 +235,19 @@ static SymPlan sym_plan(int64_t I, int64_t d, int64_t B, int world) {
 struct LocalPlan {
   int64_t ctrl;  // [0] barrier epoch, [1] error flag (zeroed once by the host, never by a step)
   int64_t xu[2], su, clu, v2u, au[2];
-  int64_t seed;  // backward seed slots, [2][Ug, d] (this rank's users) then [2][I, d] (the complete item replica)
+  int64_t seed;  // backward seed slots, [n_seed][Ug, d] (this rank's users) then [n_seed][I, d] (the complete item replica)
   int64_t v2_i;
   int64_t g_emb, g_l2, g_nce, bpr_scratch, bpr_losses, nce_losses, ar, umask, imask, cnt, nce_ws, total;
-  int64_t rows_u, rows_i, hfirst_u, hfirst_i, hwork_u, hwork_i;  // batch-row lists of the last forward layer
+  // batch-row lists of the last forward layer, per graph (cnt: 16 words per graph)
+  int64_t rows_u[3], rows_i[3], hfirst_u[3], hfirst_i[3], hwork_u[3], hwork_i[3];
+  int64_t cat, cat_id, n_cat;  // SGL's InfoNCE rows (GatherArgs)
   int64_t nce_ws_bytes;
+  int n_seed, n_graphs;
 };
 
-static LocalPlan local_plan(int64_t I, int64_t Ug, int64_t d, int64_t B, int64_t hub_u, int64_t hub_t) {
+// Every model but SGL gets the layout it always had; SGL adds a third seed slot per side, the batch-row lists of its two
+// views (whose split-row chunks must fit the graph's: hub_u / hub_t), and an InfoNCE workspace of one 2B problem.
+static LocalPlan local_plan(int model, int64_t I, int64_t Ug, int64_t d, int64_t B, int64_t hub_u, int64_t hub_t) {
   LocalPlan p;
   int64_t off = 0;
   auto take = [&](int64_t bytes) {
@@ -224,6 +255,9 @@ static LocalPlan local_plan(int64_t I, int64_t Ug, int64_t d, int64_t B, int64_t
     off += al256(bytes);
     return o;
   };
+  const bool sgl = model == SRB_MODEL_SGL;
+  p.n_seed = sgl ? 3 : 2;
+  p.n_graphs = sgl ? 3 : 1;
   const int64_t und = Ug * d * 4, ind = I * d * 4;
   p.ctrl = take(256);
   p.xu[0] = take(und);
@@ -233,7 +267,7 @@ static LocalPlan local_plan(int64_t I, int64_t Ug, int64_t d, int64_t B, int64_t
   p.v2u = take(und);
   p.au[0] = take(und);
   p.au[1] = take(und);
-  p.seed = take(2 * und + 2 * ind);  // contiguous: one scatter fills all four slots
+  p.seed = take(p.n_seed * (und + ind));  // contiguous: one scatter fills every slot
   p.v2_i = take(ind);
   p.g_emb = take(3 * B * d * 4);
   p.g_l2 = take(3 * B * d * 4);
@@ -245,15 +279,20 @@ static LocalPlan local_plan(int64_t I, int64_t Ug, int64_t d, int64_t B, int64_t
   // shard_begin_kernel clears both bitmaps and the list counters: [umask, nce_ws)
   p.umask = take(((Ug + 31) / 32) * 4 + 4);  // bitmap over this rank's local user rows
   p.imask = take(((I + 31) / 32) * 4);
-  p.cnt = take(16 * 4);
-  p.nce_ws_bytes = srb_infonce_workspace_bytes((int32_t)B, (int32_t)d, 2);
+  p.cnt = take(p.n_graphs * 16 * 4);
+  p.nce_ws_bytes = sgl ? srb_infonce_workspace_bytes((int32_t)(2 * B), (int32_t)d, 1) : srb_infonce_workspace_bytes((int32_t)B, (int32_t)d, 2);
   p.nce_ws = take(p.nce_ws_bytes);
-  p.rows_u = take(4 * B * 4);
-  p.rows_i = take(4 * 2 * B * 4);
-  p.hfirst_u = take(B * 4);
-  p.hfirst_i = take(2 * B * 4);
-  p.hwork_u = take(hub_u * 2 * 4);
-  p.hwork_i = take(hub_t * 2 * 4);
+  for (int q = 0; q < p.n_graphs; ++q) {
+    p.rows_u[q] = take(4 * B * 4);
+    p.rows_i[q] = take(4 * 2 * B * 4);
+    p.hfirst_u[q] = take(B * 4);
+    p.hfirst_i[q] = take(2 * B * 4);
+    p.hwork_u[q] = take(hub_u * 2 * 4);
+    p.hwork_i[q] = take(hub_t * 2 * 4);
+  }
+  p.cat = take(sgl ? 2 * B * 4 : 0);
+  p.cat_id = take(sgl ? 2 * B * 4 : 0);
+  p.n_cat = take(sgl ? 4 : 0);
   p.total = off;
   return p;
 }
@@ -270,8 +309,19 @@ struct Ctx {
   float* mine(int64_t off) const { return (float*)(sym + off); }
   float* lw(int64_t off) const { return (float*)(loc + off); }
   float* seed_u(int t) const { return lw(lp.seed) + (size_t)t * Ug * d; }
-  float* seed_i(int t) const { return lw(lp.seed) + ((size_t)2 * Ug + (size_t)t * I) * d; }
+  float* seed_i(int t) const { return lw(lp.seed) + ((size_t)lp.n_seed * Ug + (size_t)t * I) * d; }
 };
+
+// One graph's blocks on this rank and the index of their batch-row lists: 0 = Ru / Rt, 1 and 2 = SGL's two views
+struct Blocks {
+  const srb_graph_csr* ru;  // [Ug x I]
+  const srb_graph_csr* rt;  // [I x Ug]
+  int q;
+};
+
+static Blocks blocks(const Ctx& c, int q) {
+  return q == 0 ? Blocks{&c.s->Ru, &c.s->Rt, 0} : Blocks{&c.s->Ru_view[q - 1], &c.s->Rt_view[q - 1], q};
+}
 
 // SRB_SHARD_SYNC=barrier: separate barrier launches between the kernels of a layer instead of waits / signals folded
 // into them (measurement switch; both are kept parity-tested)
@@ -335,6 +385,9 @@ struct Epi {
   // user half (local tables) / item half (item-id indexed tables)
   float* y_u = nullptr;
   int64_t y_i = -1;            // symmetric offset of the item output (pushed to every rank) or -1
+  float* y_i_loc = nullptr;    // or: local item output, not pushed (world > 1: valid on the owner's slice only)
+  const float* extra_u = nullptr;    // dense addend of every row (the outputs' layouts), or null
+  const float* extra_i = nullptr;
   const float* sum_in_u = nullptr;
   float* sum_out_u = nullptr;
   const float* sum_in_i = nullptr;
@@ -349,7 +402,7 @@ struct Epi {
   bool rows_only = false;            // last forward layer: only the batch rows (lists of shard_batch_rows_kernel)
 };
 
-static int base_args(const Ctx& c, const srb_graph_csr& g, int n_rows, const float* X, const uint32_t* mask, SpmmArgs& a) {
+static int base_args(const Ctx& c, const srb_graph_csr& g, int n_rows, int n_cols, const float* X, const uint32_t* mask, SpmmArgs& a) {
   srb_spmm_desc p = {};
   p.rowptr = g.rowptr;
   p.colidx = g.colidx;
@@ -359,7 +412,7 @@ static int base_args(const Ctx& c, const srb_graph_csr& g, int n_rows, const flo
   p.n_vlong_rows = g.n_vlong_rows;
   p.hub = g.hub;
   p.n_rows = n_rows;
-  p.n_cols = (&g == &c.s->Ru) ? c.I : c.Ug;
+  p.n_cols = n_cols;
   p.d = c.d;
   p.X = X;
   p.col_mask = mask;
@@ -368,17 +421,16 @@ static int base_args(const Ctx& c, const srb_graph_csr& g, int n_rows, const flo
   return fill_args(&p, a);
 }
 
-// Restrict a product over one of the rank's blocks to the batch rows listed by shard_batch_rows_kernel
+// Restrict a product over block g (Ru or Rt of graph q) to the batch rows listed by shard_batch_rows_kernel
 // (device-classified list, dynamic chunk lists of the split rows; the graph's own partial-sum scratch is reused).
-static void use_batch_rows(const Ctx& c, bool item_side, SpmmArgs& a) {
-  const srb_graph_csr& g = item_side ? c.s->Rt : c.s->Ru;
+static void use_batch_rows(const Ctx& c, const srb_graph_csr& g, int q, bool item_side, SpmmArgs& a) {
   const int hcap = g.hub.n_work;
-  a.row_order = (const int32_t*)(c.loc + (item_side ? c.lp.rows_i : c.lp.rows_u));
+  a.row_order = (const int32_t*)(c.loc + (item_side ? c.lp.rows_i[q] : c.lp.rows_u[q]));
   a.n_rows = item_side ? 2 * c.B : c.B;
-  a.n_vlong_dev = (const int32_t*)(c.loc + c.lp.cnt) + (item_side ? 8 : 0);
+  a.n_vlong_dev = (const int32_t*)(c.loc + c.lp.cnt) + 16 * q + (item_side ? 8 : 0);
   a.n_huge = a.n_vlong = a.n_long = 0;
-  a.hub_first = hcap ? (const int32_t*)(c.loc + (item_side ? c.lp.hfirst_i : c.lp.hfirst_u)) : nullptr;
-  a.hub_work = hcap ? (const int32_t*)(c.loc + (item_side ? c.lp.hwork_i : c.lp.hwork_u)) : nullptr;
+  a.hub_first = hcap ? (const int32_t*)(c.loc + (item_side ? c.lp.hfirst_i[q] : c.lp.hfirst_u[q])) : nullptr;
+  a.hub_work = hcap ? (const int32_t*)(c.loc + (item_side ? c.lp.hwork_i[q] : c.lp.hwork_u[q])) : nullptr;
   a.hub_part = hcap ? g.hub.part : nullptr;
   a.n_work = hcap;
   a.seg = a.seg_cnt = a.order_cta = a.order_warp = nullptr;
@@ -405,7 +457,8 @@ static void item_epilogue(const Ctx& c, const Epi& e, SpmmArgs& a) {
   const srb_shard_desc* s = c.s;
   epi_common(c, e, a);
   a.noise_row_base = c.U;
-  a.Y = e.y_i >= 0 ? c.mine(e.y_i) : nullptr;
+  a.Y = e.y_i >= 0 ? c.mine(e.y_i) : e.y_i_loc;
+  a.extra = e.extra_i;
   a.seed = e.seed_i;  // (world > 1: added by the owner's reduction only, after the rank-ordered sum)
   a.seed_mask = (const uint32_t*)(c.loc + c.lp.imask);
   a.sum_in = e.sum_in_i;
@@ -437,14 +490,14 @@ static void item_epilogue(const Ctx& c, const Epi& e, SpmmArgs& a) {
   }
 }
 
-// One propagation layer on the sharded tables: (xu [Ug,d] local, xi [I,d] replicated) -> outputs per `e`.
-static int layer(const Ctx& c, const float* xu, const float* xi, const Epi& e) {
+// One propagation layer over the block pair bl: (xu [Ug,d] local, xi [I,d] replicated) -> outputs per `e`.
+static int layer(const Ctx& c, const Blocks& bl, const float* xu, const float* xi, const Epi& e) {
   const srb_shard_desc* s = c.s;
   // ---- item half, part 1: this rank's partial product R_g^T xu ----
   {
     SpmmArgs a;
-    SRB_TRY(base_args(c, s->Rt, c.I, xu, e.mask_u, a));
-    if (e.rows_only) use_batch_rows(c, true, a);
+    SRB_TRY(base_args(c, *bl.rt, c.I, c.Ug, xu, e.mask_u, a));
+    if (e.rows_only) use_batch_rows(c, *bl.rt, bl.q, true, a);
     if (c.G == 1) {
       item_epilogue(c, e, a);
     } else {
@@ -473,7 +526,7 @@ static int layer(const Ctx& c, const float* xu, const float* xi, const Epi& e) {
   cudaStream_t rs = overlap ? (cudaStream_t)s->fork_stream : c.st;
   auto reduce = [&]() -> int {
     SpmmArgs a;
-    SRB_TRY(base_args(c, s->Rt, c.I, xu, nullptr, a));
+    SRB_TRY(base_args(c, *bl.rt, c.I, c.Ug, xu, nullptr, a));
     item_epilogue(c, e, a);
     ReduceArgs r = {};
     r.stage = c.mine(c.sp.stage);
@@ -490,12 +543,13 @@ static int layer(const Ctx& c, const float* xu, const float* xi, const Epi& e) {
   auto user_half = [&]() -> int {
     if (c.Ug <= 0) return SRB_OK;
     SpmmArgs a;
-    SRB_TRY(base_args(c, s->Ru, c.Ug, xi, e.mask_i, a));
-    if (e.rows_only) use_batch_rows(c, false, a);
+    SRB_TRY(base_args(c, *bl.ru, c.Ug, c.I, xi, e.mask_i, a));
+    if (e.rows_only) use_batch_rows(c, *bl.ru, bl.q, false, a);
     epi_common(c, e, a);
     a.noise_row_base = c.rank;  // global id of local user row r: rank + r * world
     a.noise_row_stride = c.G;
     a.Y = e.y_u;
+    a.extra = e.extra_u;
     a.seed = e.seed_u;
     a.seed_mask = (const uint32_t*)(c.loc + c.lp.umask);
     a.sum_in = e.sum_in_u;
@@ -525,7 +579,7 @@ static int layer(const Ctx& c, const float* xu, const float* xi, const Epi& e) {
 // Encoder forward on the sharded tables (R4).  sums: running layer sum / final mean (user local, item owner slice).
 // batch_rows: training forward -- the final mean is only read at the batch rows, so the last layer skips the rest.
 // x1u / x1i: output of layer 1 evaluated by the caller (SimGCL's shared first product); the loop starts at layer 2.
-static int encoder(const Ctx& c, bool include_ego, int noise_mode, int view, int layer_cl, float* sum_u, float* sum_i,
+static int encoder(const Ctx& c, const Blocks& bl, bool include_ego, int noise_mode, int view, int layer_cl, float* sum_u, float* sum_i,
                    float* cl_u, int64_t cl_i_off, bool push_final_items, bool batch_rows, const float* x1u = nullptr,
                    const float* x1i = nullptr) {
   const srb_shard_desc* s = c.s;
@@ -555,7 +609,7 @@ static int encoder(const Ctx& c, bool include_ego, int noise_mode, int view, int
     e.sum_scale = last ? inv : 1.f;
     e.rows_only = batch_rows && last && !is_cl;  // (a CL view at the last layer is needed in full)
     if (last && push_final_items) e.sum_push_i = (int64_t)((char*)sum_i - c.sym);
-    SRB_TRY(layer(c, xu, xi, e));
+    SRB_TRY(layer(c, bl, xu, xi, e));
     if (e.y_u) {
       xu = e.y_u;
       xi = c.mine(e.y_i);
@@ -579,6 +633,12 @@ static int gather(const Ctx& c, const float* utab, const float* itab, int64_t ct
   for (int q = 0; q < c.G; ++q) g.dst[q] = c.symf(ctab_off, q);
   g.n_dst = c.G;
   g.ar = write_ar ? (int32_t*)(c.loc + c.lp.ar) : nullptr;
+  if (write_ar && c.s->model == SRB_MODEL_SGL) {
+    g.cat = (int32_t*)(c.loc + c.lp.cat);
+    g.cat_id = (int32_t*)(c.loc + c.lp.cat_id);
+    g.n_cat = (int32_t*)(c.loc + c.lp.n_cat);
+    g.n_users = c.U;
+  }
   const int slots = (sec_hi - sec_lo) * c.B;
   const int blocks = (slots + 7) / 8;
   switch (c.d) {
@@ -591,12 +651,13 @@ static int gather(const Ctx& c, const float* utab, const float* itab, int64_t ct
 
 static int make_ctx(const srb_shard_desc* s, void* stream, Ctx& c) {
   SRB_REQUIRE(s != nullptr, "shard: null desc");
-  SRB_REQUIRE(s->model == SRB_MODEL_LIGHTGCN || s->model == SRB_MODEL_SIMGCL || s->model == SRB_MODEL_XSIMGCL,
-              "shard: the sharded step covers LightGCN, SimGCL and XSimGCL (model %d)", s->model);
+  SRB_REQUIRE(s->model == SRB_MODEL_LIGHTGCN || s->model == SRB_MODEL_SIMGCL || s->model == SRB_MODEL_XSIMGCL || s->model == SRB_MODEL_SGL,
+              "shard: the sharded step covers LightGCN, SimGCL, XSimGCL and SGL (model %d)", s->model);
   SRB_REQUIRE(s->world >= 1 && s->world <= 8 && s->rank >= 0 && s->rank < s->world, "shard: bad world/rank %d/%d", s->world, s->rank);
   SRB_REQUIRE(s->d == 32 || s->d == 64 || s->d == 128, "shard: unsupported d=%d (32, 64, 128)", s->d);
   SRB_REQUIRE(s->n_users > 0 && s->n_items > 0 && s->batch_cap > 0 && s->n_layers >= 1, "shard: bad sizes");
   SRB_REQUIRE(s->noise_mode == 0 || s->noise_mode == 2, "shard: noise comes from the in-kernel Philox stream (noise_mode 2)");
+  SRB_REQUIRE(s->model != SRB_MODEL_SGL || s->noise_mode == 0, "shard: SGL adds no noise (noise_mode 0)");
   for (int g = 0; g < s->world; ++g) SRB_REQUIRE(s->sym[g] != nullptr, "shard: null symmetric region of rank %d", g);
   SRB_REQUIRE(s->Ru.rowptr && s->Ru.colidx && s->Ru.vals && s->Rt.rowptr && s->Rt.colidx && s->Rt.vals, "shard: null matrix");
   SRB_REQUIRE(s->pu && s->mu && s->vu && s->mi && s->vi && s->step_dev && s->scalars && s->losses, "shard: null pointer");
@@ -614,7 +675,7 @@ static int make_ctx(const srb_shard_desc* s, void* stream, Ctx& c) {
   c.L = s->n_layers;
   c.B = s->batch_cap;
   c.sp = sym_plan(c.I, c.d, c.B, c.G);
-  c.lp = local_plan(c.I, c.Ug, c.d, c.B, s->Ru.hub.n_work, s->Rt.hub.n_work);
+  c.lp = local_plan(s->model, c.I, c.Ug, c.d, c.B, s->Ru.hub.n_work, s->Rt.hub.n_work);
   SRB_REQUIRE(s->sym_bytes >= c.sp.total, "shard: symmetric region too small (%lld < %lld)", (long long)s->sym_bytes, (long long)c.sp.total);
   SRB_REQUIRE(s->workspace && s->workspace_bytes >= c.lp.total, "shard: workspace too small (%lld < %lld)",
               (long long)s->workspace_bytes, (long long)c.lp.total);
@@ -624,15 +685,65 @@ static int make_ctx(const srb_shard_desc* s, void* stream, Ctx& c) {
   return SRB_OK;
 }
 
+// engine.cu's run_chain on layer() over the block pair bl: seed slot f (F) enters at levels L-1 .. 1 and, with include_ego,
+// at the ego level; slot 1 (G) enters at level g_level instead (at the ego level: G only -- LightGCN's G holds F too).  The
+// first product gathers its input through the batch bitmaps.  Every rank reads only its own complete item slots, so the
+// chain needs no synchronisation beyond layer()'s: the owner's reduction adds the item seed after the rank-ordered sum.
+// The last product applies Adam, or with to_gd stores into gd (this rank's users, and the items of its own slice -- the
+// rows the last product of a later chain reads); with add_gd it adds gd first.
+static int chain(const Ctx& c, const Blocks& bl, int f, int g_level, bool include_ego, float* gd_u, float* gd_i, bool to_gd, bool add_gd) {
+  const int L = c.L;
+  const uint32_t* umask = (const uint32_t*)(c.loc + c.lp.umask);
+  const uint32_t* imask = (const uint32_t*)(c.loc + c.lp.imask);
+  auto slot = [&](int k) { return g_level == k ? 1 : f; };
+  float* au[2] = {c.lw(c.lp.au[0]), c.lw(c.lp.au[1])};
+  const float *xu = c.seed_u(slot(L)), *xi = c.seed_i(slot(L));
+  for (int k = L - 1, x = 0; k >= 1; --k, x ^= 1) {
+    Epi e;
+    e.y_u = au[x];
+    e.y_i = c.sp.ai[x];
+    e.seed_u = c.seed_u(slot(k));
+    e.seed_i = c.seed_i(slot(k));
+    if (k == L - 1) {  // the input is a seed slot: valid at the batch rows only
+      e.mask_u = umask;
+      e.mask_i = imask;
+    }
+    SRB_TRY(layer(c, bl, xu, xi, e));
+    xu = au[x];
+    xi = c.mine(c.sp.ai[x]);
+  }
+  Epi e;
+  const int s0 = g_level == 0 ? 1 : (include_ego ? f : -1);
+  e.seed_u = s0 >= 0 ? c.seed_u(s0) : nullptr;
+  e.seed_i = s0 >= 0 ? c.seed_i(s0) : nullptr;
+  if (L == 1) {
+    e.mask_u = umask;
+    e.mask_i = imask;
+  }
+  if (to_gd) {
+    e.y_u = gd_u;
+    e.y_i_loc = gd_i;
+  } else {
+    e.adam = true;
+  }
+  if (add_gd) {  // (out == extra: each row reads its addend before it stores)
+    e.extra_u = gd_u;
+    e.extra_i = gd_i;
+  }
+  return layer(c, bl, xu, xi, e);
+}
+
 }  // namespace srb
 
-extern "C" int srb_shard_plan(int32_t n_users, int32_t n_items, int32_t n_local_users, int32_t d, int32_t batch_cap, int32_t world,
-                                int32_t hub_chunks_u, int32_t hub_chunks_t, srb_shard_layout* out) {
+extern "C" int srb_shard_plan(int32_t model, int32_t n_users, int32_t n_items, int32_t n_local_users, int32_t d, int32_t batch_cap,
+                              int32_t world, int32_t hub_chunks_u, int32_t hub_chunks_t, srb_shard_layout* out) {
   SRB_REQUIRE(out && world >= 1 && world <= 8 && n_items > 0 && d > 0 && batch_cap > 0 && hub_chunks_u >= 0 && hub_chunks_t >= 0,
               "shard_plan: bad arguments");
+  SRB_REQUIRE(model == SRB_MODEL_LIGHTGCN || model == SRB_MODEL_SIMGCL || model == SRB_MODEL_XSIMGCL || model == SRB_MODEL_SGL,
+              "shard_plan: the sharded step covers LightGCN, SimGCL, XSimGCL and SGL (model %d)", model);
   const srb::SymPlan sp = srb::sym_plan(n_items, d, batch_cap, world);
   (void)n_users;  // (the local workspace only depends on the rank's own user count)
-  const srb::LocalPlan lp = srb::local_plan(n_items, n_local_users, d, batch_cap, hub_chunks_u, hub_chunks_t);
+  const srb::LocalPlan lp = srb::local_plan(model, n_items, n_local_users, d, batch_cap, hub_chunks_u, hub_chunks_t);
   out->sym_bytes = sp.total;
   out->workspace_bytes = lp.total;
   out->item_params = sp.pi;
@@ -650,16 +761,29 @@ extern "C" int srb_shard_step(const srb_shard_desc* s, void* stream) {
   const int B = c.B, d = c.d, L = c.L;
   const int32_t* hdr = s->batch;
   const int32_t *b_dev = hdr, *nu_dev = hdr + 1, *ni_dev = hdr + 2;
-  const bool xs = s->model == SRB_MODEL_XSIMGCL, sg = s->model == SRB_MODEL_SIMGCL, lg = s->model == SRB_MODEL_LIGHTGCN;
-  SRB_REQUIRE(lg || s->noise_mode == 2, "shard: SimGCL / XSimGCL need noise_mode 2");
+  const bool xs = s->model == SRB_MODEL_XSIMGCL, sg = s->model == SRB_MODEL_SIMGCL, lg = s->model == SRB_MODEL_LIGHTGCN,
+             sgl = s->model == SRB_MODEL_SGL;
+  SRB_REQUIRE(lg || sgl || s->noise_mode == 2, "shard: SimGCL / XSimGCL need noise_mode 2");
+  if (sgl) {
+    for (int v = 0; v < 2; ++v) {
+      const srb_graph_csr &ru = s->Ru_view[v], &rt = s->Rt_view[v];
+      SRB_REQUIRE(ru.rowptr && ru.colidx && ru.vals && rt.rowptr && rt.colidx && rt.vals,
+                  "shard: SGL needs the epoch's two view graphs as this rank's blocks (Ru_view / Rt_view of view %d are null)", v + 1);
+      SRB_REQUIRE(ru.hub.n_work <= s->Ru.hub.n_work && rt.hub.n_work <= s->Rt.hub.n_work,
+                  "shard: view %d has more split-row chunks (%d, %d) than the graph the plan was made for (%d, %d)", v + 1,
+                  ru.hub.n_work, rt.hub.n_work, s->Ru.hub.n_work, s->Rt.hub.n_work);
+    }
+  }
 
   uint32_t* umask = (uint32_t*)(c.loc + c.lp.umask);
   uint32_t* imask = (uint32_t*)(c.loc + c.lp.imask);
-  // seed slot t: user u at row u / world + t * Ug, item i at 2 * Ug + t * I + i; SimGCL's slot 1 holds a forward buffer
-  const SeedRows rows = {{0, c.G * c.Ug}, {2 * c.Ug, 2 * c.Ug + c.I}, c.G, c.rank};
+  // seed slot t: user u at row u / world + t * Ug, item i at n_seed * Ug + t * I + i; SimGCL's slot 1 holds a forward
+  // buffer.  SGL's cat lists users u and items U + i: the items go to every rank's item slots.
+  const int ns = c.lp.n_seed;
+  const SeedRows rows = {{0, c.G * c.Ug, 2 * c.G * c.Ug}, {ns * c.Ug, ns * c.Ug + c.I, ns * c.Ug + 2 * c.I}, c.G, c.rank, sgl ? c.U : 0};
   const int n_words = (int)((c.lp.nce_ws - c.lp.umask) / 4), threads = n_words > 3 * B * (d / 4) ? n_words : 3 * B * (d / 4);
   shard_begin_kernel<<<(threads + 255) / 256, 256, 0, st>>>(s->step_dev, s->scalars, s->lr, s->beta1, s->beta2, (int32_t*)umask, n_words,
-                                                            s->batch, B, d, c.lw(c.lp.seed), sg ? 1 : 2, rows);
+                                                            s->batch, B, d, c.lw(c.lp.seed), sg ? 1 : ns, rows);
   SRB_TRY(post_launch("shard_begin_kernel"));
   {
     BatchRowsArgs br = {};
@@ -669,20 +793,26 @@ extern "C" int srb_shard_step(const srb_shard_desc* s, void* stream) {
     br.imask = imask;
     br.world = c.G;
     br.rank = c.rank;
-    br.ru_rowptr = s->Ru.rowptr;
-    br.rt_rowptr = s->Rt.rowptr;
-    br.rows_u = (int32_t*)(c.loc + c.lp.rows_u);
-    br.rows_i = (int32_t*)(c.loc + c.lp.rows_i);
-    br.cnt = (int32_t*)(c.loc + c.lp.cnt);
-    br.hcap_u = s->Ru.hub.n_work;
-    br.hcap_i = s->Rt.hub.n_work;
-    br.hfirst_u = br.hcap_u ? (int32_t*)(c.loc + c.lp.hfirst_u) : nullptr;
-    br.hwork_u = (int32_t*)(c.loc + c.lp.hwork_u);
-    br.hfirst_i = br.hcap_i ? (int32_t*)(c.loc + c.lp.hfirst_i) : nullptr;
-    br.hwork_i = (int32_t*)(c.loc + c.lp.hwork_i);
+    br.n_graphs = c.lp.n_graphs;
+    for (int q = 0; q < c.lp.n_graphs; ++q) {
+      const Blocks bl = blocks(c, q);
+      BatchRowLists& l = br.g[q];
+      l.ru_rowptr = bl.ru->rowptr;
+      l.rt_rowptr = bl.rt->rowptr;
+      l.rows_u = (int32_t*)(c.loc + c.lp.rows_u[q]);
+      l.rows_i = (int32_t*)(c.loc + c.lp.rows_i[q]);
+      l.cnt = (int32_t*)(c.loc + c.lp.cnt) + 16 * q;
+      l.hcap_u = bl.ru->hub.n_work;
+      l.hcap_i = bl.rt->hub.n_work;
+      l.hfirst_u = l.hcap_u ? (int32_t*)(c.loc + c.lp.hfirst_u[q]) : nullptr;
+      l.hwork_u = (int32_t*)(c.loc + c.lp.hwork_u[q]);
+      l.hfirst_i = l.hcap_i ? (int32_t*)(c.loc + c.lp.hfirst_i[q]) : nullptr;
+      l.hwork_i = (int32_t*)(c.loc + c.lp.hwork_i[q]);
+    }
     shard_batch_rows_kernel<<<(3 * B + 255) / 256, 256, 0, st>>>(br);
     SRB_TRY(post_launch("shard_batch_rows_kernel"));
   }
+  const Blocks full = blocks(c, 0);
 
   // ---- forward ----
   float* su = c.lw(c.lp.su);
@@ -692,9 +822,13 @@ extern "C" int srb_shard_step(const srb_shard_desc* s, void* stream) {
   float* v2i = c.lw(c.lp.v2_i);
   const bool cl_hit = xs && s->layer_cl >= 1 && s->layer_cl <= L;
   if (lg) {
-    SRB_TRY(encoder(c, true, 0, 0, 0, su, si, nullptr, -1, false, true));
+    SRB_TRY(encoder(c, full, true, 0, 0, 0, su, si, nullptr, -1, false, true));
   } else if (xs) {
-    SRB_TRY(encoder(c, false, 2, 0, cl_hit ? s->layer_cl : 0, su, si, cl_hit ? clu : nullptr, c.sp.cl_i, false, true));
+    SRB_TRY(encoder(c, full, false, 2, 0, cl_hit ? s->layer_cl : 0, su, si, cl_hit ? clu : nullptr, c.sp.cl_i, false, true));
+  } else if (sgl) {  // three encoders with the ego layer in the mean (SGL.py:98-113), the views into SimGCL's view buffers
+    SRB_TRY(encoder(c, full, true, 0, 0, 0, su, si, nullptr, -1, false, true));
+    SRB_TRY(encoder(c, blocks(c, 1), true, 0, 0, 0, clu, c.mine(c.sp.cl_i), nullptr, -1, false, true));
+    SRB_TRY(encoder(c, blocks(c, 2), true, 0, 0, 0, v2u, v2i, nullptr, -1, false, true));
   } else if (L >= 2) {
     // layer 1 of SimGCL's three encoders is the same product (SimGCL.py:85): evaluated once into the backward
     // buffers (free until the backward pass), then perturbed per view (:87-88) -- users locally, the replicated
@@ -707,7 +841,7 @@ extern "C" int srb_shard_step(const srb_shard_desc* s, void* stream) {
       Epi e;
       e.y_u = zu;
       e.y_i = c.sp.ai[0];
-      SRB_TRY(layer(c, s->pu, c.mine(c.sp.pi), e));
+      SRB_TRY(layer(c, full, s->pu, c.mine(c.sp.pi), e));
       SRB_TRY(wait_peers(c));  // every slice of the item half has arrived
     }
     for (int v = 0; v < 2; ++v) {
@@ -716,7 +850,7 @@ extern "C" int srb_shard_step(const srb_shard_desc* s, void* stream) {
       e.poff = ((uint64_t)v << 32) | 0x10u;
       if (c.Ug > 0) {
         SpmmArgs a;
-        SRB_TRY(base_args(c, s->Ru, c.Ug, zu, nullptr, a));
+        SRB_TRY(base_args(c, s->Ru, c.Ug, c.I, zu, nullptr, a));
         epi_common(c, e, a);
         a.noise_row_base = c.rank;
         a.noise_row_stride = c.G;
@@ -724,25 +858,25 @@ extern "C" int srb_shard_step(const srb_shard_desc* s, void* stream) {
         SRB_TRY(launch_rows_epilogue(a, c.d, st));
       }
       SpmmArgs a;
-      SRB_TRY(base_args(c, s->Rt, c.I, zi, nullptr, a));
+      SRB_TRY(base_args(c, s->Rt, c.I, c.Ug, zi, nullptr, a));
       epi_common(c, e, a);
       a.noise_row_base = c.U;
       a.Y = x1i[v];
       SRB_TRY(launch_rows_epilogue(a, c.d, st));
     }
-    SRB_TRY(encoder(c, false, 0, 0, 0, su, si, nullptr, -1, false, true, zu, zi));
-    SRB_TRY(encoder(c, false, 2, 0, 0, clu, c.mine(c.sp.cl_i), nullptr, -1, false, true, x1u[0], x1i[0]));
-    SRB_TRY(encoder(c, false, 2, 1, 0, v2u, v2i, nullptr, -1, false, true, x1u[1], x1i[1]));
+    SRB_TRY(encoder(c, full, false, 0, 0, 0, su, si, nullptr, -1, false, true, zu, zi));
+    SRB_TRY(encoder(c, full, false, 2, 0, 0, clu, c.mine(c.sp.cl_i), nullptr, -1, false, true, x1u[0], x1i[0]));
+    SRB_TRY(encoder(c, full, false, 2, 1, 0, v2u, v2i, nullptr, -1, false, true, x1u[1], x1i[1]));
   } else {
-    SRB_TRY(encoder(c, false, 0, 0, 0, su, si, nullptr, -1, false, true));
-    SRB_TRY(encoder(c, false, 2, 0, 0, clu, c.mine(c.sp.cl_i), nullptr, -1, false, true));
-    SRB_TRY(encoder(c, false, 2, 1, 0, v2u, v2i, nullptr, -1, false, true));
+    SRB_TRY(encoder(c, full, false, 0, 0, 0, su, si, nullptr, -1, false, true));
+    SRB_TRY(encoder(c, full, false, 2, 0, 0, clu, c.mine(c.sp.cl_i), nullptr, -1, false, true));
+    SRB_TRY(encoder(c, full, false, 2, 1, 0, v2u, v2i, nullptr, -1, false, true));
   }
 
   // ---- the rows the batch reads -> compact tables on every rank ----
-  SRB_TRY(gather(c, su, si, c.sp.cmain, 0, 5, true));
+  SRB_TRY(gather(c, su, si, c.sp.cmain, 0, sgl ? 3 : 5, true));
   if (xs) SRB_TRY(gather(c, cl_hit ? clu : s->pu, cl_hit ? c.mine(c.sp.cl_i) : c.mine(c.sp.pi), c.sp.cv1, 3, 5, false));
-  if (sg) {
+  if (sg || sgl) {
     SRB_TRY(gather(c, clu, c.mine(c.sp.cl_i), c.sp.cv1, 3, 5, false));
     SRB_TRY(gather(c, v2u, v2i, c.sp.cv2, 3, 5, false));
   }
@@ -768,7 +902,7 @@ extern "C" int srb_shard_step(const srb_shard_desc* s, void* stream) {
     p.b = B;
     p.emb_scale = 1.f;
     p.reg = s->reg;
-    p.l2_terms = lg ? 3 : 2;
+    p.l2_terms = (lg || sgl) ? 3 : 2;  // (u, p, n): LightGCN.py:25, SGL.py:36
     p.l2_div = s->l2_div;
     p.grad_scale = 1.f;
     p.losses = bpr_losses;
@@ -797,41 +931,34 @@ extern "C" int srb_shard_step(const srb_shard_desc* s, void* stream) {
     q.workspace_bytes = c.lp.nce_ws_bytes;
     SRB_TRY(srb_infonce_fwd_bwd(&q, stream));
     n_nce = 2;
+  } else if (sgl) {  // one problem over the unique users followed by the unique items (SGL.py:120-125)
+    srb_infonce_desc q = {};
+    q.n_problems = 1;
+    q.d = d;
+    q.b_cos = 1;
+    q.temperature = s->tau;
+    q.prob[0] = {c.mine(c.sp.cv1), c.mine(c.sp.cv2), 0, 0, 1.f, 1.f, (const int32_t*)(c.loc + c.lp.cat),
+                 (const int32_t*)(c.loc + c.lp.n_cat), 2 * B, s->cl_rate, g1a, g1b, nce_losses + 0};
+    q.workspace = c.loc + c.lp.nce_ws;
+    q.workspace_bytes = c.lp.nce_ws_bytes;
+    SRB_TRY(srb_infonce_fwd_bwd(&q, stream));
+    n_nce = 1;
   }
   SRB_TRY(finalize_losses(bpr_losses, nce_losses, n_nce, s->cl_rate, s->losses, st));
 
-  // ---- backward: engine.cu's Horner chain (run_chain) on layer() + Adam ----
-  // Seed slots F (0) and G (1): slot g_level == k at level k.  Every rank reads only its own complete item slots, so the
-  // chain needs no synchronisation beyond layer()'s: the owner's reduction adds the item seed after the rank-ordered sum.
-  const SeedGrads gr = {s->batch, B, d, g_emb, g_l2, {g1a, g2a}, {g1b, g2b}, nullptr, nullptr};
+  // ---- backward: engine.cu's Horner chains on layer() + Adam ----
+  const SeedGrads gr = {s->batch, B, d, g_emb, g_l2, {g1a, sgl ? g1b : g2a}, {g1b, g2b}, sgl ? (const int32_t*)(c.loc + c.lp.cat_id) : nullptr,
+                        sgl ? (const int32_t*)(c.loc + c.lp.n_cat) : nullptr};
   ScatterSegs segs = {};
   const int g_level = seed_segments(s->model, L, s->layer_cl, gr, rows, segs);
   SRB_TRY(scatter_segments(c.lw(c.lp.seed), d, segs, st));
-  float* au[2] = {c.lw(c.lp.au[0]), c.lw(c.lp.au[1])};
-  const float *xu = c.seed_u(g_level == L), *xi = c.seed_i(g_level == L);
-  for (int k = L - 1, x = 0; k >= 1; --k, x ^= 1) {
-    Epi e;
-    e.y_u = au[x];
-    e.y_i = c.sp.ai[x];
-    e.seed_u = c.seed_u(g_level == k);
-    e.seed_i = c.seed_i(g_level == k);
-    if (k == L - 1) {  // the input is a seed slot: valid at the batch rows only
-      e.mask_u = umask;
-      e.mask_i = imask;
-    }
-    SRB_TRY(layer(c, xu, xi, e));
-    xu = au[x];
-    xi = c.mine(c.sp.ai[x]);
-  }
-  Epi e;
-  e.adam = true;
-  e.seed_u = g_level == 0 ? c.seed_u(1) : nullptr;  // the ego level takes G only (LightGCN's G holds F too)
-  e.seed_i = g_level == 0 ? c.seed_i(1) : nullptr;
-  if (L == 1) {
-    e.mask_u = umask;
-    e.mask_i = imask;
-  }
-  return layer(c, xu, xi, e);
+  if (!sgl) return chain(c, full, 0, g_level, lg, nullptr, nullptr, false, false);
+  // SGL's three graphs differ: the two view chains sum into gd, then the graph's chain adds it and applies Adam.  gd is a
+  // local table (view 2's forward buffers, free once gathered) and is never pushed: its item rows are only read by this
+  // rank's reduction of its own slice.
+  SRB_TRY(chain(c, blocks(c, 1), 0, -1, true, v2u, v2i, true, false));
+  SRB_TRY(chain(c, blocks(c, 2), 1, -1, true, v2u, v2i, true, true));
+  return chain(c, full, 2, -1, true, v2u, v2i, false, true);
 }
 
 /* Clean forward for evaluation / save() (XSimGCL.py:40-41, 53-55): the final mean of this rank's users goes to
@@ -842,7 +969,7 @@ extern "C" int srb_shard_forward(const srb_shard_desc* s, float* out_user, void*
   Ctx c;
   SRB_TRY(make_ctx(s, stream, c));
   SRB_REQUIRE(out_user != nullptr || c.Ug == 0, "shard_forward: null output");
-  const bool ego = s->model == SRB_MODEL_LIGHTGCN;
-  SRB_TRY(encoder(c, ego, 0, 0, 0, out_user, c.mine(c.sp.fin_i), nullptr, -1, true, false));
+  const bool ego = s->model == SRB_MODEL_LIGHTGCN || s->model == SRB_MODEL_SGL;
+  SRB_TRY(encoder(c, blocks(c, 0), ego, 0, 0, 0, out_user, c.mine(c.sp.fin_i), nullptr, -1, true, false));
   return wait_peers(c);  // every slice of the item output has arrived
 }

@@ -12,9 +12,11 @@ def max_rel(a, b):
     return float((a - b).abs().max().item()) / max(den, 1e-30)
 
 
-def sharded_vs_single(model, data, d, L, B, batches, *, steps=3, lr=1e-3, reg=1e-4, seed=7, dev=None, multicast=None, nvls=None, **kw):
+def sharded_vs_single(model, data, d, L, B, batches, *, steps=3, lr=1e-3, reg=1e-4, seed=7, dev=None, multicast=None, nvls=None, views=None,
+                      **kw):
     """Collective over the default process group (or single-process).  Runs `steps` steps of ShardedEngine on all
-    ranks and of TrainEngine on every rank (the reference replica), on batches[k] (device int32 rows).
+    ranks and of TrainEngine on every rank (the reference replica), on batches[k] (device int32 rows).  views: SGL's two
+    view graphs, given to both engines.
     Returns dict(loss_rel, m_*_rel, v_*_rel, final_*_rel, user_rel, item_rel, upd_off_frac, max_rel, ...) -- maxima
     over steps and ranks; max_rel covers the losses, the Adam moments and the clean forward."""
     import torch
@@ -28,6 +30,9 @@ def sharded_vs_single(model, data, d, L, B, batches, *, steps=3, lr=1e-3, reg=1e
     ii = torch.empty((I, d), device=dev).uniform_(-0.1, 0.1, generator=g)
     sh = ShardedEngine(model, data, d, L, B, lr, reg, init_user=iu, init_item=ii, philox_seed=seed, device=dev, multicast=multicast, nvls=nvls, **kw)
     ref = TrainEngine(model, data, d, L, B, lr, reg, init_user=iu, init_item=ii, philox_seed=seed, device=dev, **kw)
+    if views is not None:
+        sh.set_view_graphs(*views)
+        ref.set_view_graphs(*views)
     # Parity is asserted on well-conditioned quantities: the losses, Adam's first moment m (linear in the gradient:
     # after step 1, m = 0.1 g) and second moment, and the clean forward.  The PARAMETERS themselves are compared in two
     # ways that say what they mean: relative to the table (`user_rel` / `item_rel`), and as the fraction of entries

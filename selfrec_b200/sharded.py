@@ -74,20 +74,20 @@ def extract_blocks(rowptr, colidx, vals, n_users, n_items, rank, world):
 
 
 class ShardedEngine:
-    """LightGCN / SimGCL / XSimGCL training on bipartite-sharded tables; world == 1 works without torch.distributed.
+    """LightGCN / SimGCL / XSimGCL / SGL training on bipartite-sharded tables; world == 1 works without torch.distributed.
 
     Same constructor surface as TrainEngine.  Every rank must feed the SAME batch buffer to step().  Parameters:
     `user_emb` = this rank's users [Ug, d] (global ids `user_ids`: rank, rank + world, ...), `item_emb` = the full
     replicated [I, d] item table.  The in-kernel Philox noise is keyed by global row ids, so a sharded run with the same
-    philox_seed draws the noise the single-GPU TrainEngine draws."""
+    philox_seed draws the noise the single-GPU TrainEngine draws.  SGL needs set_view_graphs() once per epoch."""
 
     def __init__(self, model, data, emb_size, n_layers, batch_size, lr, reg, *, eps=0.0, tau=0.2, cl_rate=0.0, layer_cl=0,
                  l2_div=1.0, init_user=None, init_item=None, group=None, philox_seed=0x5EED, device=None, multicast=None, nvls=None):
         import torch
         from . import ops
         lib = _lib.require_device()
-        if model not in ("LightGCN", "SimGCL", "XSimGCL"):
-            raise _lib.SrbError("the sharded engine covers LightGCN, SimGCL and XSimGCL")
+        if model not in ("LightGCN", "SimGCL", "XSimGCL", "SGL"):
+            raise _lib.SrbError("the sharded engine covers LightGCN, SimGCL, XSimGCL and SGL")
         if int(emb_size) not in ops._SUPPORTED_D:
             raise _lib.SrbError(f"embedding.size {emb_size} is not supported by the CUDA path {ops._SUPPORTED_D}")
         self.torch, self.ops, self.lib = torch, ops, lib
@@ -125,7 +125,8 @@ class ShardedEngine:
         # ---- memory ----
         lay = _lib.ShardLayout()
         gu, gt = self.Ru.graph_struct(self.d), self.Rt.graph_struct(self.d)
-        _lib.check(lib.srb_shard_plan(self.U, self.I, self.Ug, self.d, self.B, self.world, int(gu.hub.n_work), int(gt.hub.n_work),
+        self.hub_cap = (int(gu.hub.n_work), int(gt.hub.n_work))  # split-row chunk capacity of the batch-row lists (SGL: views too)
+        _lib.check(lib.srb_shard_plan(_lib.MODEL_IDS[model], self.U, self.I, self.Ug, self.d, self.B, self.world, *self.hub_cap,
                                       C.byref(lay)), "srb_shard_plan")
         self.layout = lay
         self.sym_handle = None
@@ -184,7 +185,7 @@ class ShardedEngine:
         s.n_users, s.n_items, s.d, s.n_layers, s.batch_cap, s.layer_cl = self.U, self.I, self.d, self.L, self.B, int(layer_cl)
         s.eps, s.tau, s.cl_rate, s.reg = float(eps), float(tau), float(cl_rate), float(reg)
         s.lr, s.beta1, s.beta2, s.adam_eps, s.l2_div = float(lr), 0.9, 0.999, 1e-8, float(l2_div)
-        s.noise_mode = 2 if model in ("SimGCL", "XSimGCL") else 0
+        s.noise_mode = 2 if model in ("SimGCL", "XSimGCL") else 0  # (LightGCN, SGL: none)
         s.philox_seed = int(philox_seed)
         s.Ru, s.Rt = gu, gt
         p = ops._p
@@ -207,10 +208,50 @@ class ShardedEngine:
         s.nvls = 1 if (want_nvls and mc_ptr) else 0
         self.use_nvls = bool(s.nvls)
         self.desc = s
+        self.view_blocks = None
         self.graph = None
         self._warm = False
         torch.cuda.synchronize()
         self._host_barrier()
+
+    # ---- configuration -------------------------------------------------------------------
+    def set_view_graphs(self, adj1, adj2):
+        """SGL: the epoch's two dropped, re-normalised (U+I)^2 graphs (SGL.py:27-29; e.g. DeviceBipartite.assemble output),
+        drawn identically on every rank.  Keeps this rank's Ru / Rt blocks of each; the full views are not kept.  Drops a
+        captured graph (capture() again, on every rank)."""
+        torch, ops = self.torch, self.ops
+        if self.model_name != "SGL":
+            raise _lib.SrbError(f"set_view_graphs: {self.model_name} has no view graphs")
+        views = []
+        for k, a in enumerate((adj1, adj2)):
+            a = a if isinstance(a, ops.SparseAdj) else ops.SparseAdj(a)
+            if tuple(a.shape) != (self.N, self.N):
+                raise ValueError(f"set_view_graphs: view {k + 1} is {tuple(a.shape)}, the graph is {(self.N, self.N)}")
+            a.cuda(self.dev)
+            ru, rt = extract_blocks(a.rowptr, a.colidx, a.vals, self.U, self.I, self.rank, self.world)
+            bru = ops.SparseAdj.from_device(*ru, (self.Ug, self.I), symmetric=False)
+            brt = ops.SparseAdj.from_device(*rt, (self.I, self.Ug), symmetric=False)
+            gu, gt = bru.graph_struct(self.d), brt.graph_struct(self.d)
+            if gu.hub.n_work > self.hub_cap[0] or gt.hub.n_work > self.hub_cap[1]:
+                raise _lib.SrbError(f"set_view_graphs: view {k + 1} has more split-row chunks ({gu.hub.n_work}, {gt.hub.n_work}) than "
+                                    f"the graph the workspace was planned for ({self.hub_cap[0]}, {self.hub_cap[1]})")
+            views.append((a, bru, brt, gu, gt))
+        if self.dist is not None and self.world > 1:
+            # every rank must have drawn the same views: their nnz and a position-weighted sum of their column indices
+            sig = []
+            for a, *_ in views:
+                w = torch.arange(a.nnz, device=self.dev, dtype=torch.int64) % 65521 + 1
+                sig += [a.nnz, int((a.colidx.to(torch.int64) * w).sum().item())]
+            t = torch.tensor(sig + [-x for x in sig], dtype=torch.int64,
+                             device=self.dev if self.dist.get_backend(self.group) == "nccl" else "cpu")
+            self.dist.all_reduce(t, op=self.dist.ReduceOp.MAX, group=self.group)
+            hi, lo = t[: len(sig)].tolist(), [-x for x in t[len(sig):].tolist()]
+            if hi != lo:
+                raise _lib.SrbError("set_view_graphs: the ranks drew different view graphs (seed every rank's `random` alike)")
+        self.view_blocks = [(bru, brt) for _a, bru, brt, _gu, _gt in views]
+        for k, (_a, _bru, _brt, gu, gt) in enumerate(views):
+            self.desc.Ru_view[k], self.desc.Rt_view[k] = gu, gt
+        self.graph = None  # pointers changed: a captured graph is stale
 
     # ---- plumbing ------------------------------------------------------------------------
     def _host_barrier(self):
