@@ -4,6 +4,7 @@
 #include <stdint.h>
 #include <stdio.h>
 #include <atomic>
+#include <functional>
 #include <utility>
 #include "selfrec_b200.h"
 
@@ -109,8 +110,37 @@ struct SeedGrads {  // a batch's compact loss gradients, [cap, d] per batch list
 };
 // Which gradient enters which table, with what scale (one scatter); returns the level where G enters, or -1 (run_chain)
 int seed_segments(int model, int n_layers, int layer_cl, const SeedGrads& g, const SeedRows& r, ScatterSegs& segs);
-// a step's four losses (BPR, L2, cl_rate x the sum of n_nce InfoNCE losses, total) into out[4] (engine.cu)
-int finalize_losses(const float* bpr_losses, const float* nce_losses, int n_nce, float cl_rate, float* out, cudaStream_t st);
+// First kernel of a graph model's step (engine.cu): Adam's bias corrections, words[0, n_words) cleared, and the batch rows
+// of the first n_seed seed tables cleared on layout r
+int step_begin(int32_t* step, float* scalars, double lr, double b1, double b2, int32_t* words, int n_words, const int32_t* batch, int cap,
+               int d, float* seed, int n_seed, const SeedRows& r, cudaStream_t st);
+
+// The loss stage of both training steps (engine.cu), on [rows, d] tables: the step's output, the raw E0 (LightGCN's L2
+// term), view 1 (XSimGCL: the CL view) and view 2.
+struct LossRows {
+  const int32_t* batch;              // SRB_BATCH_HEADER counts: b, unique users, unique items (then seed_segments' lists)
+  const int32_t *u, *i, *j;          // BPR: table rows u, item_off + i, item_off + j
+  int32_t item_off;
+  const int32_t *uq_u, *uq_i;        // InfoNCE: table rows uq_off[0] + unique user, uq_off[1] + unique item
+  int32_t uq_off[2];
+  const int32_t *cat, *n_cat;        // SGL's one InfoNCE problem: table rows of the unique users, then of the unique items
+  const int32_t* cat_id;             // the same entries as ids u | U + i (SeedGrads.cat)
+};
+struct LossBufs {
+  float *g_emb, *g_l2;               // [3][cap, d]
+  float* g_nce;                      // InfoNCE gradients: view v of problem p at g_nce + (2p + v) * nce_plane; SGL's one
+  size_t nce_plane;                  // problem of 2 cap rows: view v at g_nce + 2v * cap * d
+  float *bpr_scratch, *bpr_losses, *nce_losses;
+  void* nce_ws;
+  int64_t nce_ws_bytes;
+  float* losses;                     // [4]
+};
+struct ForkRes;  // engine.cu: with one, BPR + L2 run on its side stream beside the InfoNCE
+// BPR + L2, the model's InfoNCE (before_nce, if set, is enqueued on st just before it) and the step's four losses (BPR,
+// L2, cl_rate x the InfoNCE losses, total) into o.losses; g gets the gradients where they were written (seed_segments)
+int step_losses(int model, float reg, float l2_div, float tau, float cl_rate, int d, int cap, const float* out, const float* e0,
+                const float* v1, const float* v2, const LossRows& r, const LossBufs& o, ForkRes* fork,
+                const std::function<int()>& before_nce, SeedGrads& g, cudaStream_t st);
 
 // Adam step counter + bias corrections in double, like torch's Python floats (one thread)
 __device__ __forceinline__ void adam_prepare(int32_t* step, float* scalars, double lr, double b1, double b2) {

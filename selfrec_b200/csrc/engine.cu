@@ -179,24 +179,38 @@ __global__ void __launch_bounds__(256) build_batch_rows_kernel(const int32_t* ba
   list_batch_row(row, rowptr[row + 1] - rowptr[row], 0, rows, 3 * cap, counters, hub_first, hub_work, hub_cap);
 }
 
-// first kernel of a graph model's step: Adam's bias corrections, the batch-row counters + bitmap cleared, and the batch
-// rows u, U + i, U + j of the n_seed [N, d] seed tables cleared, a float4 per thread (duplicates only repeat a store).
-// One node instead of a kernel and two memsets.
+// first kernel of a graph model's step (both training steps): Adam's bias corrections, n_words words cleared (the
+// batch-row counters + bitmaps), and the batch rows u, i, j of the first n_seed seed tables cleared where the seed
+// scatter puts them (layout r), a float4 per thread (duplicates only repeat a store).  One node instead of a kernel and
+// two memsets.  OWNED: r has cyclic user ownership (r.user_mod > 0: the sharded step).  A compile-time switch: with the
+// ownership test and division behind a runtime flag, the single-GPU step's kernel took 3.26 us instead of 2.88 us
+// (yelp2018 XSimGCL, H100 80GB HBM3, 700 W).
+template <bool OWNED>
 __global__ void __launch_bounds__(256) step_begin_kernel(int32_t* step, float* scalars, double lr, double b1, double b2, int32_t* words,
-                                                         int n_words, const int32_t* batch, int cap, int n_users, int n, int d,
-                                                         float* seed, int n_seed) {
+                                                         int n_words, const int32_t* batch, int cap, int d, float* seed, int n_seed,
+                                                         const SeedRows r) {
   pdl_wait();
   pdl_trigger();
   const int t = blockIdx.x * blockDim.x + threadIdx.x;
   if (t == 0) adam_prepare(step, scalars, lr, b1, b2);
   if (t < n_words) words[t] = 0;
-  const int per_row = d / 4;
-  const int r = t / per_row, c = (t % per_row) * 4;
-  const int sec = r / cap, k = r % cap;
+  const int k0 = t / (d / 4), c = (t % (d / 4)) * 4;
+  const int sec = k0 / cap, k = k0 % cap;
   if (sec >= 3 || k >= min(batch[0], cap)) return;
-  const int32_t* u = batch + SRB_BATCH_HEADER;
-  const size_t row = (sec == 0) ? u[k] : n_users + u[sec * cap + k];
-  for (int q = 0; q < n_seed; ++q) st4(seed + ((size_t)q * n + row) * d + c, f4_zero());
+  const int id = batch[SRB_BATCH_HEADER + sec * cap + k];
+  const bool owned = OWNED && sec == 0;  // local row (id + user_off) / user_mod
+  if (owned && id % r.user_mod != r.user_rem) return;  // another rank's user
+  for (int q = 0; q < n_seed; ++q) {
+    const int row = id + (sec == 0 ? r.user_off[q] : r.item_off[q]);
+    st4(seed + (size_t)(owned ? row / r.user_mod : row) * d + c, f4_zero());
+  }
+}
+
+int step_begin(int32_t* step, float* scalars, double lr, double b1, double b2, int32_t* words, int n_words, const int32_t* batch, int cap,
+               int d, float* seed, int n_seed, const SeedRows& r, cudaStream_t st) {
+  const int threads = std::max(n_words, 3 * cap * (d / 4));
+  return launch_kernel(r.user_mod > 0 ? step_begin_kernel<true> : step_begin_kernel<false>, (threads + 255) / 256, 256, 0, st,
+                       "step_begin_kernel", step, scalars, lr, b1, b2, words, n_words, batch, cap, d, seed, n_seed, r);
 }
 
 __global__ void finalize_losses_kernel(const float* bpr_losses, const float* nce_losses, int n_nce, float cl_rate, float* out) {
@@ -209,10 +223,6 @@ __global__ void finalize_losses_kernel(const float* bpr_losses, const float* nce
   out[1] = bpr_losses[1];
   out[2] = cl;
   out[3] = bpr_losses[0] + bpr_losses[1] + cl;
-}
-
-int finalize_losses(const float* bpr_losses, const float* nce_losses, int n_nce, float cl_rate, float* out, cudaStream_t st) {
-  return launch_kernel(finalize_losses_kernel, 1, 1, 0, st, "finalize_losses_kernel", bpr_losses, nce_losses, n_nce, cl_rate, out);
 }
 
 int seed_segments(int model, int n_layers, int layer_cl, const SeedGrads& g, const SeedRows& r, ScatterSegs& segs) {
@@ -272,35 +282,24 @@ int seed_segments(int model, int n_layers, int layer_cl, const SeedGrads& g, con
 static int spmm_simple(const srb_step_desc* s, const srb_graph_csr* g, const float* x, float* y, const float* extra,
                        bool adam, cudaStream_t st, const uint32_t* col_mask = nullptr, const float* seed = nullptr,
                        const uint32_t* seed_mask = nullptr) {
-  srb_spmm_desc p = {};
-  p.col_mask = col_mask;
-  p.rowptr = g->rowptr;
-  p.colidx = g->colidx;
-  p.vals = g->vals;
-  p.row_order = g->row_order;
-  p.n_long_rows = g->n_long_rows;
-  p.n_vlong_rows = g->n_vlong_rows;
-  p.hub = g->hub;
-  p.n_rows = p.n_cols = s->n_users + s->n_items;
-  p.d = s->d;
-  p.X = x;
-  p.Y = y;
-  p.extra = extra;
-  p.extra_scale = 1.f;
-  if (adam) {
-    p.adam_p = s->params;
-    p.adam_m = s->adam_m;
-    p.adam_v = s->adam_v;
-    p.adam_scalars = s->scalars;
-    p.beta1 = s->beta1;
-    p.beta2 = s->beta2;
-    p.adam_eps = s->adam_eps;
-  }
   SpmmArgs a;
-  SRB_TRY(fill_args(&p, a));
+  SRB_TRY(graph_args(*g, s->n_users + s->n_items, s->n_users + s->n_items, s->d, x, a));
+  a.col_mask = col_mask;
+  a.Y = y;
+  a.extra = extra;
   a.seed_mask = seed_mask;
   a.seed = seed;
-  return launch_spmm(a, p.d, st);
+  if (adam) {
+    a.ap = s->params;
+    a.am = s->adam_m;
+    a.av = s->adam_v;
+    a.ascal = s->scalars;
+    a.b2 = (float)s->beta2;
+    a.w1 = (float)(1.0 - s->beta1);
+    a.w2 = (float)(1.0 - s->beta2);
+    a.aeps = s->adam_eps;
+  }
+  return launch_spmm(a, s->d, st);
 }
 
 // BPR + L2 and InfoNCE only read the encoder outputs and write disjoint buffers: the step forks BPR onto a
@@ -335,6 +334,72 @@ static ForkRes* fork_res(const srb_step_desc* s, ForkRes* own) {
     r.ok = true;
   }
   return &r;
+}
+
+int step_losses(int model, float reg, float l2_div, float tau, float cl_rate, int d, int cap, const float* out, const float* e0,
+                const float* v1, const float* v2, const LossRows& r, const LossBufs& o, ForkRes* fork,
+                const std::function<int()>& before_nce, SeedGrads& g, cudaStream_t st) {
+  const bool lg = model == SRB_MODEL_LIGHTGCN, xs = model == SRB_MODEL_XSIMGCL, sg = model == SRB_MODEL_SIMGCL;
+  if (fork) {
+    SRB_TRY(check_cuda(cudaEventRecord(fork->fork, st), "fork record"));
+    SRB_TRY(check_cuda(cudaStreamWaitEvent(fork->side, fork->fork, 0), "fork wait"));
+  }
+  srb_bpr_desc p = {};
+  p.emb = out;
+  p.l2_emb = lg ? e0 : out;  // LightGCN.py:25 regularises the raw parameters
+  p.n_users = r.item_off;
+  p.d = d;
+  p.u_idx = r.u;
+  p.i_idx = r.i;
+  p.j_idx = r.j;
+  p.b_dev = r.batch;
+  p.b = cap;
+  p.emb_scale = 1.f;
+  p.reg = reg;
+  // (u,p,n)/batch_size: MF.py:21, LightGCN.py:25 | (u,p): SimGCL.py:31, XSimGCL.py:33 | (u,p,n): SGL.py:36
+  p.l2_terms = (sg || xs) ? 2 : 3;
+  p.l2_div = l2_div;
+  p.grad_scale = 1.f;
+  p.losses = o.bpr_losses;
+  p.g_emb = o.g_emb;
+  p.g_l2 = lg ? o.g_l2 : nullptr;
+  p.scratch = o.bpr_scratch;
+  SRB_TRY(srb_bpr_l2_fwd_bwd(&p, fork ? fork->side : st));
+  if (fork) SRB_TRY(check_cuda(cudaEventRecord(fork->join, fork->side), "join record"));
+  if (before_nce) SRB_TRY(before_nce());
+
+  g = SeedGrads{r.batch, cap, d, o.g_emb, p.g_l2, {}, {}, nullptr, nullptr};
+  srb_infonce_desc q = {};
+  q.d = d;
+  q.b_cos = 1;
+  q.temperature = tau;
+  q.workspace = o.nce_ws;
+  q.workspace_bytes = o.nce_ws_bytes;
+  if (xs || sg) {  // users and items: XSimGCL contrasts the output with its CL view, SimGCL its two views
+    const float* t1 = xs ? out : v1;
+    const float* t2 = xs ? v1 : v2;
+    float* gp[4];
+    for (int k = 0; k < 4; ++k) gp[k] = o.g_nce + k * o.nce_plane;
+    q.n_problems = 2;
+    q.prob[0] = {t1, t2, r.uq_off[0], r.uq_off[0], 1.f, 1.f, r.uq_u, r.batch + 1, cap, cl_rate, gp[0], gp[1], o.nce_losses + 0};
+    q.prob[1] = {t1, t2, r.uq_off[1], r.uq_off[1], 1.f, 1.f, r.uq_i, r.batch + 2, cap, cl_rate, gp[2], gp[3], o.nce_losses + 1};
+    g.nce_u[0] = gp[0];
+    g.nce_u[1] = gp[1];
+    g.nce_i[0] = gp[2];
+    g.nce_i[1] = gp[3];
+  } else if (model == SRB_MODEL_SGL) {  // one problem over cat(users, items) (SGL.py:120-125)
+    float* g2 = o.g_nce + (size_t)2 * cap * d;
+    q.n_problems = 1;
+    q.prob[0] = {v1, v2, 0, 0, 1.f, 1.f, r.cat, r.n_cat, 2 * cap, cl_rate, o.g_nce, g2, o.nce_losses + 0};
+    g.nce_u[0] = o.g_nce;
+    g.nce_u[1] = g2;
+    g.cat = r.cat_id;
+    g.n_cat = r.n_cat;
+  }
+  if (q.n_problems) SRB_TRY(srb_infonce_fwd_bwd(&q, st));
+  if (fork) SRB_TRY(check_cuda(cudaStreamWaitEvent(st, fork->join, 0), "join wait"));
+  return launch_kernel(finalize_losses_kernel, 1, 1, 0, st, "finalize_losses_kernel", o.bpr_losses, o.nce_losses, q.n_problems, cl_rate,
+                       o.losses);
 }
 
 // The Horner backward chain of one encoder on graph g.  Its loss gradients were scattered beforehand into [N, d] seed
@@ -384,7 +449,7 @@ static int encoder(const srb_step_desc* s, const Ws& w, const srb_graph_csr* g, 
   if (noise_mode == 1) e.noise = s->noise + (size_t)view * s->n_layers * e.n * e.d;
   e.eps = s->eps;
   e.philox_seed = s->philox_seed;
-  e.philox_offset = ((uint64_t)view << 32) | 0x10u;
+  e.philox_offset = noise_offset(view, 0);  // (+ layer in srb_encoder_forward)
   e.philox_step_dev = s->step_dev;
   e.E0 = s->params;
   if (cl_out && layer_cl == s->n_layers) {
@@ -407,24 +472,18 @@ static int encoder(const srb_step_desc* s, const Ws& w, const srb_graph_csr* g, 
 // out = x + sign(x) * normalize(noise) * eps, row by row: the noise one perturbed SimGCL encoder adds to the shared
 // first product (SimGCL.py:87-88), drawn exactly as the fused SpMM epilogue of layer 1 of view `view` would draw it.
 static int perturb_rows(const srb_step_desc* s, const float* x, float* out, int view, cudaStream_t st) {
-  const size_t nd = (size_t)(s->n_users + s->n_items) * s->d;
-  srb_spmm_desc p = {};
-  p.rowptr = s->adj.rowptr;  // (not read by the epilogue-only kernel)
-  p.colidx = s->adj.colidx;
-  p.vals = s->adj.vals;
-  p.n_rows = p.n_cols = s->n_users + s->n_items;
-  p.d = s->d;
-  p.X = x;
-  p.Y = out;
-  p.extra_scale = 1.f;
-  p.sum_scale = 1.f;
-  p.noise_mode = s->noise_mode;
-  if (s->noise_mode == 1) p.noise = s->noise + (size_t)view * s->n_layers * nd;
-  p.eps = s->eps;
-  p.philox_seed = s->philox_seed;
-  p.philox_offset = ((uint64_t)view << 32) | 0x10u;
-  p.philox_step_dev = s->step_dev;
-  return srb_spmm_epilogue_rows(&p, st);
+  const int N = s->n_users + s->n_items;
+  SpmmArgs a;
+  SRB_TRY(graph_args(s->adj, N, N, s->d, x, a));  // (the graph is not read by the epilogue-only kernel)
+  a.Y = out;
+  a.noise_mode = s->noise_mode;
+  if (s->noise_mode == 1) a.noise = s->noise + (size_t)view * s->n_layers * N * s->d;
+  a.eps = s->eps;
+  const uint64_t poff = noise_offset(view, 0);
+  a.pkey = make_uint2((uint32_t)s->philox_seed, (uint32_t)(s->philox_seed >> 32));
+  a.poff = make_uint2((uint32_t)poff, (uint32_t)(poff >> 32));
+  a.pstep = s->step_dev;
+  return launch_rows_epilogue(a, s->d, st);
 }
 
 }  // namespace srb
@@ -458,31 +517,26 @@ extern "C" int srb_train_step(const srb_step_desc* s, void* stream) {
   carve(s, &w, (char*)s->workspace);
   cudaStream_t st = (cudaStream_t)stream;
   const int B = s->batch_cap, d = s->d, U = s->n_users, L = s->n_layers;
-  const int32_t* hdr = s->batch;
   const int32_t* u_idx = s->batch + SRB_BATCH_HEADER;
   const int32_t* i_idx = u_idx + B;
   const int32_t* j_idx = i_idx + B;
   const int32_t* uq_u = j_idx + B;
   const int32_t* uq_i = uq_u + B;
-  const int32_t* b_dev = hdr + 0;
-  const int32_t* nu_dev = hdr + 1;
-  const int32_t* ni_dev = hdr + 2;
+  const int32_t* b_dev = s->batch;
+  const SeedRows rows = {{0, N, 2 * N}, {U, N + U, 2 * N + U}, 0, 0};  // seed table t: rows t * N + [0, N)
 
   PdlScope pdl;
 
   // ---- forward ----
   if (s->model != SRB_MODEL_MF) {
     const int n_words = 8 + (U + s->n_items + 31) / 32;  // [class counters | row bitmap]
-    const int threads = std::max(n_words, 3 * B * (d / 4));
-    SRB_TRY(launch_kernel(step_begin_kernel, (threads + 255) / 256, 256, 0, st, "step_begin_kernel", s->step_dev, s->scalars, s->lr,
-                          s->beta1, s->beta2, w.n_hub, n_words, s->batch, B, U, N, d, w.seed, w.n_seed));
+    SRB_TRY(step_begin(s->step_dev, s->scalars, s->lr, s->beta1, s->beta2, w.n_hub, n_words, s->batch, B, d, w.seed, w.n_seed, rows, st));
     SRB_TRY(launch_kernel(build_batch_rows_kernel, (3 * B + 255) / 256, 256, 0, st, "build_batch_rows_kernel", s->batch, B, U, s->adj.rowptr,
                           w.batch_rows, w.n_hub, w.row_mask, w.hub_cap ? w.hub_first : nullptr, w.hub_work, w.hub_cap));
   } else {
     SRB_TRY(srb_adam_prepare(s->step_dev, s->scalars, s->lr, s->beta1, s->beta2, stream));
   }
   const float* table = s->params;  // table BPR gathers from
-  int n_nce = 0;
   switch (s->model) {
     case SRB_MODEL_MF: break;
     case SRB_MODEL_LIGHTGCN:
@@ -523,73 +577,16 @@ extern "C" int srb_train_step(const srb_step_desc* s, void* stream) {
       break;
   }
 
-  // ---- BPR + L2 (on the side stream when an InfoNCE follows) ----
+  // ---- BPR + L2 (on the side stream when an InfoNCE follows), InfoNCE ----
   ForkRes fk_own = {};
   ForkRes* fk = (s->model == SRB_MODEL_XSIMGCL || s->model == SRB_MODEL_SIMGCL || s->model == SRB_MODEL_SGL) ? fork_res(s, &fk_own) : nullptr;
-  if (fk) {
-    SRB_TRY(check_cuda(cudaEventRecord(fk->fork, st), "fork record"));
-    SRB_TRY(check_cuda(cudaStreamWaitEvent(fk->side, fk->fork, 0), "fork wait"));
-  }
-  {
-    srb_bpr_desc p = {};
-    p.emb = table;
-    p.l2_emb = (s->model == SRB_MODEL_LIGHTGCN) ? s->params : table;  // LightGCN.py:25 regularises raw params
-    p.n_users = U;
-    p.d = d;
-    p.u_idx = u_idx;
-    p.i_idx = i_idx;
-    p.j_idx = j_idx;
-    p.b_dev = b_dev;
-    p.b = B;
-    p.emb_scale = 1.f;
-    p.reg = s->reg;
-    // (u,p,n)/batch_size: MF.py:21, LightGCN.py:25 | (u,p): SimGCL.py:31, XSimGCL.py:33 | (u,p,n): SGL.py:36
-    p.l2_terms = (s->model == SRB_MODEL_SIMGCL || s->model == SRB_MODEL_XSIMGCL) ? 2 : 3;
-    p.l2_div = s->l2_div;
-    p.grad_scale = 1.f;
-    p.losses = w.bpr_losses;
-    p.g_emb = w.g_emb;
-    p.g_l2 = (s->model == SRB_MODEL_LIGHTGCN) ? w.g_l2 : nullptr;
-    p.scratch = w.bpr_scratch;
-    SRB_TRY(srb_bpr_l2_fwd_bwd(&p, fk ? (void*)fk->side : stream));
-    if (fk) SRB_TRY(check_cuda(cudaEventRecord(fk->join, fk->side), "join record"));
-  }
-
-  // ---- InfoNCE ----
-  const size_t gn = (size_t)2 * B * d;
-  float* g1a = w.g_nce;
-  float* g2a = w.g_nce + gn;
-  float* g1b = w.g_nce + 2 * gn;
-  float* g2b = w.g_nce + 3 * gn;
-  if (s->model == SRB_MODEL_XSIMGCL || s->model == SRB_MODEL_SIMGCL) {
-    srb_infonce_desc q = {};
-    q.n_problems = 2;
-    q.d = d;
-    q.b_cos = 1;
-    q.temperature = s->tau;
-    const float* t1 = (s->model == SRB_MODEL_XSIMGCL) ? w.final_ : w.cl;
-    const float* t2 = (s->model == SRB_MODEL_XSIMGCL) ? w.cl : w.v2;
-    q.prob[0] = {t1, t2, 0, 0, 1.f, 1.f, uq_u, nu_dev, B, s->cl_rate, g1a, g2a, w.nce_losses + 0};
-    q.prob[1] = {t1, t2, U, U, 1.f, 1.f, uq_i, ni_dev, B, s->cl_rate, g1b, g2b, w.nce_losses + 1};
-    q.workspace = w.nce_ws;
-    q.workspace_bytes = w.nce_ws_bytes;
-    SRB_TRY(srb_infonce_fwd_bwd(&q, stream));
-    n_nce = 2;
-  } else if (s->model == SRB_MODEL_SGL) {
-    SRB_TRY(launch_kernel(build_cat_idx_kernel, 8, 256, 0, st, "build_cat_idx_kernel", s->batch, B, U, w.idx_cat, w.n_cat));
-    srb_infonce_desc q = {};
-    q.n_problems = 1;
-    q.d = d;
-    q.b_cos = 1;
-    q.temperature = s->tau;
-    q.prob[0] = {w.cl, w.v2, 0, 0, 1.f, 1.f, w.idx_cat, w.n_cat, 2 * B, s->cl_rate, g1a, g2a, w.nce_losses + 0};
-    q.workspace = w.nce_ws;
-    q.workspace_bytes = w.nce_ws_bytes;
-    SRB_TRY(srb_infonce_fwd_bwd(&q, stream));
-    n_nce = 1;
-  }
-  if (fk) SRB_TRY(check_cuda(cudaStreamWaitEvent(st, fk->join, 0), "join wait"));
-  SRB_TRY(finalize_losses(w.bpr_losses, w.nce_losses, n_nce, s->cl_rate, s->losses, st));
+  std::function<int()> build_cat;  // SGL: the cat list on the main stream, after the fork (BPR does not wait for it)
+  if (s->model == SRB_MODEL_SGL)
+    build_cat = [&] { return launch_kernel(build_cat_idx_kernel, 8, 256, 0, st, "build_cat_idx_kernel", s->batch, B, U, w.idx_cat, w.n_cat); };
+  const LossRows lr = {s->batch, u_idx, i_idx, j_idx, U, uq_u, uq_i, {0, U}, w.idx_cat, w.n_cat, w.idx_cat};
+  const LossBufs lb = {w.g_emb, w.g_l2, w.g_nce, (size_t)2 * B * d, w.bpr_scratch, w.bpr_losses, w.nce_losses, w.nce_ws, w.nce_ws_bytes, s->losses};
+  SeedGrads gr;
+  SRB_TRY(step_losses(s->model, s->reg, s->l2_div, s->tau, s->cl_rate, d, B, table, s->params, w.cl, w.v2, lr, lb, fk, build_cat, gr, st));
 
   // ---- backward + Adam ----
   const size_t plane = (size_t)B * d;
@@ -606,8 +603,6 @@ extern "C" int srb_train_step(const srb_step_desc* s, void* stream) {
                          stream);
   }
   auto seed_table = [&](int t) { return w.seed + (size_t)t * N * d; };
-  const SeedGrads gr = {s->batch, B, d, w.g_emb, w.g_l2, {g1a, g2a}, {g1b, g2b}, w.idx_cat, w.n_cat};
-  const SeedRows rows = {{0, N, 2 * N}, {U, N + U, 2 * N + U}, 0, 0};  // seed table t: rows t * N + [0, N)
   ScatterSegs sg = {};
   const int g_level = seed_segments(s->model, L, s->layer_cl, gr, rows, sg);
   SRB_TRY(scatter_segments(w.seed, d, sg, st));

@@ -67,30 +67,13 @@ __global__ void shard_barrier_kernel(const BarrierArgs b) {
   }
 }
 
-// First kernel of the step (engine.cu's step_begin_kernel on this layout): Adam's bias corrections, n_words words cleared,
-// and the batch rows u, i, j of the first n_seed seed slots cleared where the seed scatter puts them, a float4 per thread.
-__global__ void __launch_bounds__(256) shard_begin_kernel(int32_t* step, float* scalars, double lr, double b1, double b2, int32_t* words,
-                                                          int n_words, const int32_t* batch, int cap, int d, float* seed, int n_seed,
-                                                          const SeedRows r) {
-  const int t = blockIdx.x * blockDim.x + threadIdx.x;
-  if (t == 0) adam_prepare(step, scalars, lr, b1, b2);
-  if (t < n_words) words[t] = 0;
-  const int k0 = t / (d / 4), c = (t % (d / 4)) * 4;
-  const int sec = k0 / cap, k = k0 % cap;
-  if (sec >= 3 || k >= min(batch[0], cap)) return;
-  const int id = batch[SRB_BATCH_HEADER + sec * cap + k];
-  if (sec == 0 && id % r.user_mod != r.user_rem) return;  // another rank's user
-  for (int q = 0; q < n_seed; ++q)
-    st4(seed + (size_t)(sec == 0 ? (id + r.user_off[q]) / r.user_mod : id + r.item_off[q]) * d + c, f4_zero());
-}
-
 // Bits of the batch's (local) users / items (masks of the row-sparse first backward product: umask over this rank's
 // local user rows, imask over all items), and -- from the thread that sets
 // a bit first, so every row is listed once -- the batch's rows of this rank's two blocks, classified by degree for the
 // last forward layer (nothing but the batch rows of the final mean is read): local users -> rows of Ru, items ->
 // rows of Rt.  Lists follow srb_spmm_desc.n_vlong_dev: four segments (split, CTA, warp, lane group -- unused) of
 // capacity cap (users) / 2 * cap (items); cnt[0..3] class sizes and cnt[4] chunks of the user list, cnt[8..] of the
-// item list.  cnt and both bitmaps are zeroed by shard_begin_kernel.
+// item list.  cnt and both bitmaps are zeroed by step_begin_kernel.
 // SGL's three graphs share the batch rows and the bitmaps but not the degrees: the same thread lists the row for each.
 struct BatchRowLists {  // one graph's lists
   const int32_t* ru_rowptr;
@@ -276,7 +259,7 @@ static LocalPlan local_plan(int model, int64_t I, int64_t Ug, int64_t d, int64_t
   p.bpr_losses = take(2 * 4);
   p.nce_losses = take(4 * 4);
   p.ar = take(2 * B * 4);
-  // shard_begin_kernel clears both bitmaps and the list counters: [umask, nce_ws)
+  // step_begin_kernel clears both bitmaps and the list counters: [umask, nce_ws)
   p.umask = take(((Ug + 31) / 32) * 4 + 4);  // bitmap over this rank's local user rows
   p.imask = take(((I + 31) / 32) * 4);
   p.cnt = take(p.n_graphs * 16 * 4);
@@ -402,25 +385,6 @@ struct Epi {
   bool rows_only = false;            // last forward layer: only the batch rows (lists of shard_batch_rows_kernel)
 };
 
-static int base_args(const Ctx& c, const srb_graph_csr& g, int n_rows, int n_cols, const float* X, const uint32_t* mask, SpmmArgs& a) {
-  srb_spmm_desc p = {};
-  p.rowptr = g.rowptr;
-  p.colidx = g.colidx;
-  p.vals = g.vals;
-  p.row_order = g.row_order;
-  p.n_long_rows = g.n_long_rows;
-  p.n_vlong_rows = g.n_vlong_rows;
-  p.hub = g.hub;
-  p.n_rows = n_rows;
-  p.n_cols = n_cols;
-  p.d = c.d;
-  p.X = X;
-  p.col_mask = mask;
-  p.extra_scale = 1.f;
-  p.sum_scale = 1.f;
-  return fill_args(&p, a);
-}
-
 // Restrict a product over block g (Ru or Rt of graph q) to the batch rows listed by shard_batch_rows_kernel
 // (device-classified list, dynamic chunk lists of the split rows; the graph's own partial-sum scratch is reused).
 static void use_batch_rows(const Ctx& c, const srb_graph_csr& g, int q, bool item_side, SpmmArgs& a) {
@@ -496,7 +460,8 @@ static int layer(const Ctx& c, const Blocks& bl, const float* xu, const float* x
   // ---- item half, part 1: this rank's partial product R_g^T xu ----
   {
     SpmmArgs a;
-    SRB_TRY(base_args(c, *bl.rt, c.I, c.Ug, xu, e.mask_u, a));
+    SRB_TRY(graph_args(*bl.rt, c.I, c.Ug, c.d, xu, a));
+    a.col_mask = e.mask_u;
     if (e.rows_only) use_batch_rows(c, *bl.rt, bl.q, true, a);
     if (c.G == 1) {
       item_epilogue(c, e, a);
@@ -526,7 +491,7 @@ static int layer(const Ctx& c, const Blocks& bl, const float* xu, const float* x
   cudaStream_t rs = overlap ? (cudaStream_t)s->fork_stream : c.st;
   auto reduce = [&]() -> int {
     SpmmArgs a;
-    SRB_TRY(base_args(c, *bl.rt, c.I, c.Ug, xu, nullptr, a));
+    SRB_TRY(graph_args(*bl.rt, c.I, c.Ug, c.d, xu, a));
     item_epilogue(c, e, a);
     ReduceArgs r = {};
     r.stage = c.mine(c.sp.stage);
@@ -543,7 +508,8 @@ static int layer(const Ctx& c, const Blocks& bl, const float* xu, const float* x
   auto user_half = [&]() -> int {
     if (c.Ug <= 0) return SRB_OK;
     SpmmArgs a;
-    SRB_TRY(base_args(c, *bl.ru, c.Ug, c.I, xi, e.mask_i, a));
+    SRB_TRY(graph_args(*bl.ru, c.Ug, c.I, c.d, xi, a));
+    a.col_mask = e.mask_i;
     if (e.rows_only) use_batch_rows(c, *bl.ru, bl.q, false, a);
     epi_common(c, e, a);
     a.noise_row_base = c.rank;  // global id of local user row r: rank + r * world
@@ -593,7 +559,7 @@ static int encoder(const Ctx& c, const Blocks& bl, bool include_ego, int noise_m
     const bool is_cl = cl_u && layer_cl == k + 1;
     Epi e;
     e.noise_mode = noise_mode;
-    e.poff = ((uint64_t)view << 32) | (uint64_t)(0x10 + k);
+    e.poff = noise_offset(view, k);
     if (is_cl) {
       e.y_u = cl_u;
       e.y_i = cl_i_off;
@@ -759,8 +725,6 @@ extern "C" int srb_shard_step(const srb_shard_desc* s, void* stream) {
   SRB_REQUIRE(s->batch != nullptr, "shard: null batch");
   cudaStream_t st = c.st;
   const int B = c.B, d = c.d, L = c.L;
-  const int32_t* hdr = s->batch;
-  const int32_t *b_dev = hdr, *nu_dev = hdr + 1, *ni_dev = hdr + 2;
   const bool xs = s->model == SRB_MODEL_XSIMGCL, sg = s->model == SRB_MODEL_SIMGCL, lg = s->model == SRB_MODEL_LIGHTGCN,
              sgl = s->model == SRB_MODEL_SGL;
   SRB_REQUIRE(lg || sgl || s->noise_mode == 2, "shard: SimGCL / XSimGCL need noise_mode 2");
@@ -781,10 +745,8 @@ extern "C" int srb_shard_step(const srb_shard_desc* s, void* stream) {
   // buffer.  SGL's cat lists users u and items U + i: the items go to every rank's item slots.
   const int ns = c.lp.n_seed;
   const SeedRows rows = {{0, c.G * c.Ug, 2 * c.G * c.Ug}, {ns * c.Ug, ns * c.Ug + c.I, ns * c.Ug + 2 * c.I}, c.G, c.rank, sgl ? c.U : 0};
-  const int n_words = (int)((c.lp.nce_ws - c.lp.umask) / 4), threads = n_words > 3 * B * (d / 4) ? n_words : 3 * B * (d / 4);
-  shard_begin_kernel<<<(threads + 255) / 256, 256, 0, st>>>(s->step_dev, s->scalars, s->lr, s->beta1, s->beta2, (int32_t*)umask, n_words,
-                                                            s->batch, B, d, c.lw(c.lp.seed), sg ? 1 : ns, rows);
-  SRB_TRY(post_launch("shard_begin_kernel"));
+  SRB_TRY(step_begin(s->step_dev, s->scalars, s->lr, s->beta1, s->beta2, (int32_t*)umask, (int)((c.lp.nce_ws - c.lp.umask) / 4), s->batch, B,
+                     d, c.lw(c.lp.seed), sg ? 1 : ns, rows, st));
   {
     BatchRowsArgs br = {};
     br.batch = s->batch;
@@ -847,10 +809,10 @@ extern "C" int srb_shard_step(const srb_shard_desc* s, void* stream) {
     for (int v = 0; v < 2; ++v) {
       Epi e;
       e.noise_mode = 2;
-      e.poff = ((uint64_t)v << 32) | 0x10u;
+      e.poff = noise_offset(v, 0);
       if (c.Ug > 0) {
         SpmmArgs a;
-        SRB_TRY(base_args(c, s->Ru, c.Ug, c.I, zu, nullptr, a));
+        SRB_TRY(graph_args(s->Ru, c.Ug, c.I, c.d, zu, a));
         epi_common(c, e, a);
         a.noise_row_base = c.rank;
         a.noise_row_stride = c.G;
@@ -858,7 +820,7 @@ extern "C" int srb_shard_step(const srb_shard_desc* s, void* stream) {
         SRB_TRY(launch_rows_epilogue(a, c.d, st));
       }
       SpmmArgs a;
-      SRB_TRY(base_args(c, s->Rt, c.I, c.Ug, zi, nullptr, a));
+      SRB_TRY(graph_args(s->Rt, c.I, c.Ug, c.d, zi, a));
       epi_common(c, e, a);
       a.noise_row_base = c.U;
       a.Y = x1i[v];
@@ -883,72 +845,18 @@ extern "C" int srb_shard_step(const srb_shard_desc* s, void* stream) {
   if (lg) SRB_TRY(gather(c, s->pu, c.mine(c.sp.pi), c.sp.cp, 0, 3, false));
   SRB_TRY(barrier(c));
 
-  // ---- BPR + L2, InfoNCE on the compact tables (replicated) ----
+  // ---- BPR + L2, InfoNCE on the compact tables (replicated); serial: the fork stream belongs to layer() ----
+  // compact rows: u at k, i at B + k, j at 2B + k, unique users at 3B + k, unique items at 4B + k
   const int32_t* ar = (const int32_t*)(c.loc + c.lp.ar);
-  float* g_emb = c.lw(c.lp.g_emb);
-  float* g_l2 = c.lw(c.lp.g_l2);
-  float* bpr_losses = c.lw(c.lp.bpr_losses);
-  float* nce_losses = c.lw(c.lp.nce_losses);
-  {
-    srb_bpr_desc p = {};
-    p.emb = c.mine(c.sp.cmain);
-    p.l2_emb = lg ? c.mine(c.sp.cp) : p.emb;  // LightGCN.py:25 regularises the raw parameters
-    p.n_users = B;                             // compact layout: u rows [0, B), i rows [B, 2B), j rows [2B, 3B)
-    p.d = d;
-    p.u_idx = ar;
-    p.i_idx = ar;
-    p.j_idx = ar + B;
-    p.b_dev = b_dev;
-    p.b = B;
-    p.emb_scale = 1.f;
-    p.reg = s->reg;
-    p.l2_terms = (lg || sgl) ? 3 : 2;  // (u, p, n): LightGCN.py:25, SGL.py:36
-    p.l2_div = s->l2_div;
-    p.grad_scale = 1.f;
-    p.losses = bpr_losses;
-    p.g_emb = g_emb;
-    p.g_l2 = lg ? g_l2 : nullptr;
-    p.scratch = c.lw(c.lp.bpr_scratch);
-    SRB_TRY(srb_bpr_l2_fwd_bwd(&p, stream));
-  }
-  const size_t plane = (size_t)B * d;
-  float* g1a = c.lw(c.lp.g_nce);
-  float* g2a = g1a + plane;
-  float* g1b = g1a + 2 * plane;
-  float* g2b = g1a + 3 * plane;
-  int n_nce = 0;
-  if (xs || sg) {
-    srb_infonce_desc q = {};
-    q.n_problems = 2;
-    q.d = d;
-    q.b_cos = 1;
-    q.temperature = s->tau;
-    const float* t1 = xs ? c.mine(c.sp.cmain) : c.mine(c.sp.cv1);
-    const float* t2 = xs ? c.mine(c.sp.cv1) : c.mine(c.sp.cv2);
-    q.prob[0] = {t1, t2, 3 * B, 3 * B, 1.f, 1.f, ar, nu_dev, B, s->cl_rate, g1a, g2a, nce_losses + 0};
-    q.prob[1] = {t1, t2, 4 * B, 4 * B, 1.f, 1.f, ar, ni_dev, B, s->cl_rate, g1b, g2b, nce_losses + 1};
-    q.workspace = c.loc + c.lp.nce_ws;
-    q.workspace_bytes = c.lp.nce_ws_bytes;
-    SRB_TRY(srb_infonce_fwd_bwd(&q, stream));
-    n_nce = 2;
-  } else if (sgl) {  // one problem over the unique users followed by the unique items (SGL.py:120-125)
-    srb_infonce_desc q = {};
-    q.n_problems = 1;
-    q.d = d;
-    q.b_cos = 1;
-    q.temperature = s->tau;
-    q.prob[0] = {c.mine(c.sp.cv1), c.mine(c.sp.cv2), 0, 0, 1.f, 1.f, (const int32_t*)(c.loc + c.lp.cat),
-                 (const int32_t*)(c.loc + c.lp.n_cat), 2 * B, s->cl_rate, g1a, g1b, nce_losses + 0};
-    q.workspace = c.loc + c.lp.nce_ws;
-    q.workspace_bytes = c.lp.nce_ws_bytes;
-    SRB_TRY(srb_infonce_fwd_bwd(&q, stream));
-    n_nce = 1;
-  }
-  SRB_TRY(finalize_losses(bpr_losses, nce_losses, n_nce, s->cl_rate, s->losses, st));
+  const LossRows lr = {s->batch, ar, ar, ar + B, B, ar, ar, {3 * B, 4 * B}, (const int32_t*)(c.loc + c.lp.cat),
+                       (const int32_t*)(c.loc + c.lp.n_cat), (const int32_t*)(c.loc + c.lp.cat_id)};
+  const LossBufs lb = {c.lw(c.lp.g_emb), c.lw(c.lp.g_l2), c.lw(c.lp.g_nce), (size_t)B * d, c.lw(c.lp.bpr_scratch), c.lw(c.lp.bpr_losses),
+                       c.lw(c.lp.nce_losses), c.loc + c.lp.nce_ws, c.lp.nce_ws_bytes, s->losses};
+  SeedGrads gr;
+  SRB_TRY(step_losses(s->model, s->reg, s->l2_div, s->tau, s->cl_rate, d, B, c.mine(c.sp.cmain), c.mine(c.sp.cp), c.mine(c.sp.cv1),
+                      c.mine(c.sp.cv2), lr, lb, nullptr, nullptr, gr, st));
 
   // ---- backward: engine.cu's Horner chains on layer() + Adam ----
-  const SeedGrads gr = {s->batch, B, d, g_emb, g_l2, {g1a, sgl ? g1b : g2a}, {g1b, g2b}, sgl ? (const int32_t*)(c.loc + c.lp.cat_id) : nullptr,
-                        sgl ? (const int32_t*)(c.loc + c.lp.n_cat) : nullptr};
   ScatterSegs segs = {};
   const int g_level = seed_segments(s->model, L, s->layer_cl, gr, rows, segs);
   SRB_TRY(scatter_segments(c.lw(c.lp.seed), d, segs, st));

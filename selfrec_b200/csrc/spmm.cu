@@ -726,6 +726,24 @@ int fill_args(const srb_spmm_desc* d, SpmmArgs& a) {
   return SRB_OK;
 }
 
+int graph_args(const srb_graph_csr& g, int n_rows, int n_cols, int d, const float* X, SpmmArgs& a) {
+  srb_spmm_desc p = {};
+  p.rowptr = g.rowptr;
+  p.colidx = g.colidx;
+  p.vals = g.vals;
+  p.row_order = g.row_order;
+  p.n_long_rows = g.n_long_rows;
+  p.n_vlong_rows = g.n_vlong_rows;
+  p.hub = g.hub;
+  p.n_rows = n_rows;
+  p.n_cols = n_cols;
+  p.d = d;
+  p.X = X;
+  p.extra_scale = 1.f;
+  p.sum_scale = 1.f;
+  return fill_args(&p, a);
+}
+
 }  // namespace srb
 
 extern "C" int srb_spmm_csr(const srb_spmm_desc* desc, void* stream) {

@@ -146,6 +146,11 @@ int launch_spmm(const SpmmArgs& a, int d, cudaStream_t st);
 int launch_reduce_rows(const SpmmArgs& a, const ReduceArgs& r, int d, cudaStream_t st);
 int launch_rows_epilogue(const SpmmArgs& a, int d, cudaStream_t st);  // Y[r] = epilogue(X[r]), r < n_rows
 int fill_args(const srb_spmm_desc* d, SpmmArgs& a);
+// the product Y = g X (g: n_rows x n_cols) with a neutral epilogue (scales 1; no output, noise, sum or Adam yet)
+int graph_args(const srb_graph_csr& g, int n_rows, int n_cols, int d, const float* X, SpmmArgs& a);
+
+// Philox offset of the noise that layer `layer` (0-based) of view `view` adds: both training steps draw the same stream
+inline uint64_t noise_offset(int view, int layer) { return ((uint64_t)view << 32) | (uint64_t)(0x10 + layer); }
 
 // Appends one batch row of degree deg to a device-classified row list of the last forward layer (the format of
 // srb_spmm_desc.n_vlong_dev): rows holds four segments of capacity cap -- split rows (only with hub_first; their

@@ -28,6 +28,60 @@ class LossHandle:
         return self._buf.numpy().copy()
 
 
+def fill_step_fields(desc, model, n_users, n_items, d, n_layers, batch_cap, *, lr, reg, eps, tau, cl_rate, layer_cl, l2_div,
+                     philox_seed):
+    """The model, shape and hyperparameter fields that srb_step_desc and srb_shard_desc share."""
+    desc.model, desc.n_users, desc.n_items, desc.d, desc.n_layers = _lib.MODEL_IDS[model], n_users, n_items, d, n_layers
+    desc.batch_cap, desc.layer_cl = batch_cap, int(layer_cl)
+    desc.eps, desc.tau, desc.cl_rate, desc.reg = float(eps), float(tau), float(cl_rate), float(reg)
+    desc.lr, desc.beta1, desc.beta2, desc.adam_eps = float(lr), 0.9, 0.999, 1e-8
+    desc.l2_div = float(l2_div)
+    desc.noise_mode = 2 if model in ("SimGCL", "XSimGCL") else 0  # in-kernel Philox noise (MF, LightGCN, SGL: none)
+    desc.philox_seed = int(philox_seed)
+
+
+def fork_resources(desc, device):
+    """A side stream and two events of the engine's own, set as desc.fork_stream / fork_event / join_event, so that two
+    engines on one device never share events.  Returns (stream, events): the caller keeps them alive."""
+    stream = torch.cuda.Stream(device=device)
+    events = (torch.cuda.Event(), torch.cuda.Event())
+    for ev in events:
+        ev.record(stream)  # torch creates the CUDA event lazily, on first record
+    desc.fork_stream = C.c_void_p(stream.cuda_stream)
+    desc.fork_event, desc.join_event = (C.c_void_p(ev.cuda_event) for ev in events)
+    return stream, events
+
+
+def capture_step(enqueue, state, warm, warmups, barrier=lambda: None):
+    """CUDA graph of one enqueue().  Unless `warm`, first runs `warmups` eager steps outside the capture (lazy module
+    load, smem attributes).  A warm-up IS a training step on whatever the batch buffer holds: the tensors in `state`
+    (parameters, moments, the step counter that keys Adam's bias correction and the Philox stream) are put back
+    afterwards, so capturing never changes the training trajectory.  `barrier` keeps the ranks of a multi-process
+    engine together around the warm-up, the restore and the capture."""
+    torch.cuda.synchronize()
+    if not warm:
+        saved = [t.clone() for t in state]
+        barrier()
+        side = torch.cuda.Stream()
+        side.wait_stream(torch.cuda.current_stream())
+        with torch.cuda.stream(side):
+            for _ in range(warmups):
+                enqueue()
+        torch.cuda.current_stream().wait_stream(side)
+        torch.cuda.synchronize()
+        barrier()
+        for dst, src in zip(state, saved):
+            dst.copy_(src)
+        del saved
+        torch.cuda.synchronize()
+        barrier()
+    g = torch.cuda.CUDAGraph()
+    with torch.cuda.graph(g):
+        enqueue()
+    barrier()
+    return g
+
+
 class TrainEngine:
     def __init__(self, model, data, emb_size, n_layers, batch_size, lr, reg, *, eps=0.0, tau=0.2, cl_rate=0.0,
                  layer_cl=0, l2_div=1.0, device=None, init_user=None, init_item=None, philox_seed=0x5EED):
@@ -85,25 +139,14 @@ class TrainEngine:
         self.view_adj = [None, None]
         self.noise = None
         s = _lib.StepDesc()
-        s.model, s.n_users, s.n_items, s.d, s.n_layers = self.model_id, self.U, self.I, self.d, self.L
-        s.batch_cap, s.layer_cl = self.B, int(layer_cl)
-        s.eps, s.tau, s.cl_rate, s.reg = float(eps), float(tau), float(cl_rate), float(reg)
-        s.lr, s.beta1, s.beta2, s.adam_eps = float(lr), 0.9, 0.999, 1e-8
-        s.l2_div = float(l2_div)
-        s.noise_mode = 2 if model in ("SimGCL", "XSimGCL") else 0
-        s.philox_seed = int(philox_seed)
+        fill_step_fields(s, model, self.U, self.I, self.d, self.L, self.B, lr=lr, reg=reg, eps=eps, tau=tau, cl_rate=cl_rate,
+                         layer_cl=layer_cl, l2_div=l2_div, philox_seed=philox_seed)
         if self.adj is not None:
             s.adj = self.adj.graph_struct(self.d)
         s.batch, s.params, s.adam_m, s.adam_v = ops._p(self.batch_dev), ops._p(self.params), ops._p(self.m), ops._p(self.v)
         s.step_dev, s.scalars, s.losses = ops._p(self.step_dev), ops._p(self.scalars), ops._p(self.losses)
         s.workspace, s.workspace_bytes = C.c_void_p(ws_ptr), ws_bytes
-        # this engine's own fork / join resources (BPR beside InfoNCE): two engines on one device never share events
-        self._fork_stream = torch.cuda.Stream(device=self.dev)
-        self._fork_events = (torch.cuda.Event(), torch.cuda.Event())
-        for ev in self._fork_events:
-            ev.record(self._fork_stream)  # torch creates the CUDA event lazily, on first record
-        s.fork_stream = C.c_void_p(self._fork_stream.cuda_stream)
-        s.fork_event, s.join_event = (C.c_void_p(ev.cuda_event) for ev in self._fork_events)
+        self._fork_stream, self._fork_events = fork_resources(s, self.dev)  # BPR beside InfoNCE
         self.desc = s
         self.eps, self.layer_cl = float(eps), int(layer_cl)
         self.sampler = None
@@ -181,29 +224,9 @@ class TrainEngine:
 
     def capture(self):
         """CUDA graph of one step on the resident batch buffer; replay with graph.replay()."""
-        torch.cuda.synchronize()
-        if not self._warm:
-            # warm-up outside capture (lazy module load, smem attributes).  A warm-up IS a training step on whatever
-            # batch_dev holds: parameters, moments and the step counter (Adam bias correction, Philox stream) are
-            # put back afterwards, so capturing never changes the training trajectory.
-            saved = (self.params.clone(), self.m.clone(), self.v.clone(), self.step_dev.clone(), self.losses.clone())
-            side = torch.cuda.Stream()
-            side.wait_stream(torch.cuda.current_stream())
-            with torch.cuda.stream(side):
-                for _ in range(2):
-                    self._enqueue()
-            torch.cuda.current_stream().wait_stream(side)
-            torch.cuda.synchronize()
-            for dst, src in zip((self.params, self.m, self.v, self.step_dev, self.losses), saved):
-                dst.copy_(src)
-            del saved
-            torch.cuda.synchronize()
-            self._warm = True
-        g = torch.cuda.CUDAGraph()
-        with torch.cuda.graph(g):
-            self._enqueue()
-        self.graph = g
-        return g
+        self.graph = capture_step(self._enqueue, (self.params, self.m, self.v, self.step_dev, self.losses), self._warm, 2)
+        self._warm = True
+        return self.graph
 
     def batches(self, exact_lazy=False):
         """One epoch of batch words from the native sampler (advances Python's `random`).  The yielded buffer is

@@ -85,6 +85,7 @@ class ShardedEngine:
                  l2_div=1.0, init_user=None, init_item=None, group=None, philox_seed=0x5EED, device=None, multicast=None, nvls=None):
         import torch
         from . import ops
+        from .engine import fill_step_fields, fork_resources
         lib = _lib.require_device()
         if model not in ("LightGCN", "SimGCL", "XSimGCL", "SGL"):
             raise _lib.SrbError("the sharded engine covers LightGCN, SimGCL, XSimGCL and SGL")
@@ -181,12 +182,9 @@ class ShardedEngine:
         self.words = _lib.BATCH_HEADER + 5 * self.B
         self.batch_dev = torch.zeros(self.words, dtype=torch.int32, device=dev)
         s = _lib.ShardDesc()
-        s.model, s.world, s.rank = _lib.MODEL_IDS[model], self.world, self.rank
-        s.n_users, s.n_items, s.d, s.n_layers, s.batch_cap, s.layer_cl = self.U, self.I, self.d, self.L, self.B, int(layer_cl)
-        s.eps, s.tau, s.cl_rate, s.reg = float(eps), float(tau), float(cl_rate), float(reg)
-        s.lr, s.beta1, s.beta2, s.adam_eps, s.l2_div = float(lr), 0.9, 0.999, 1e-8, float(l2_div)
-        s.noise_mode = 2 if model in ("SimGCL", "XSimGCL") else 0  # (LightGCN, SGL: none)
-        s.philox_seed = int(philox_seed)
+        fill_step_fields(s, model, self.U, self.I, self.d, self.L, self.B, lr=lr, reg=reg, eps=eps, tau=tau, cl_rate=cl_rate,
+                         layer_cl=layer_cl, l2_div=l2_div, philox_seed=philox_seed)
+        s.world, s.rank = self.world, self.rank
         s.Ru, s.Rt = gu, gt
         p = ops._p
         s.batch, s.pu, s.mu, s.vu, s.mi, s.vi = p(self.batch_dev), p(self.user_emb), p(self.mu), p(self.vu), p(self.mi), p(self.vi)
@@ -198,12 +196,7 @@ class ShardedEngine:
         s.workspace, s.workspace_bytes = C.c_void_p(ws_ptr), int(lay.workspace_bytes)
         if self.world > 1 and os.environ.get("SRB_SHARD_OVERLAP", "1") != "0":
             # the owner-side reduction of a layer runs on this stream beside the user-side product
-            self._fork_stream = torch.cuda.Stream(device=dev)
-            self._fork_events = (torch.cuda.Event(), torch.cuda.Event())
-            for ev in self._fork_events:
-                ev.record(self._fork_stream)  # torch creates the CUDA event lazily, on first record
-            s.fork_stream = C.c_void_p(self._fork_stream.cuda_stream)
-            s.fork_event, s.join_event = (C.c_void_p(ev.cuda_event) for ev in self._fork_events)
+            self._fork_stream, self._fork_events = fork_resources(s, dev)
         want_nvls = (os.environ.get("SRB_SHARD_NVLS", "0") == "1") if nvls is None else bool(nvls)
         s.nvls = 1 if (want_nvls and mc_ptr) else 0
         self.use_nvls = bool(s.nvls)
@@ -292,31 +285,11 @@ class ShardedEngine:
 
     def capture(self):
         """CUDA graph of one step (device-side barriers included).  Collective: every rank must call it."""
-        torch = self.torch
-        torch.cuda.synchronize()
+        from .engine import capture_step
         state = (self.user_emb, self.item_emb, self.mu, self.vu, self.mi, self.vi, self.step_dev, self.losses)
-        if not self._warm:  # a warm-up is a real step: put the trajectory back afterwards (all ranks do the same)
-            saved = [t.clone() for t in state]
-            self._host_barrier()
-            side = torch.cuda.Stream()
-            side.wait_stream(torch.cuda.current_stream())
-            with torch.cuda.stream(side):
-                self._enqueue()
-            torch.cuda.current_stream().wait_stream(side)
-            torch.cuda.synchronize()
-            self._host_barrier()
-            for dst, src in zip(state, saved):
-                dst.copy_(src)
-            del saved
-            torch.cuda.synchronize()
-            self._host_barrier()
-            self._warm = True
-        g = torch.cuda.CUDAGraph()
-        with torch.cuda.graph(g):
-            self._enqueue()
-        self.graph = g
-        self._host_barrier()
-        return g
+        self.graph = capture_step(self._enqueue, state, self._warm, 1, self._host_barrier)
+        self._warm = True
+        return self.graph
 
     # ---- inference -------------------------------------------------------------------------
     def forward_clean(self):
