@@ -14,6 +14,7 @@ import numpy as np
 import torch
 
 from .. import ops
+from ..shard_rank import is_main_process
 from ..data.loader import FileIO
 from ..data.ui_graph import Interaction
 from ..util.evaluation import ranking_evaluation, ranking_evaluation_from_masks
@@ -21,6 +22,8 @@ from .recommender import Recommender
 
 
 class GraphRecommender(Recommender):
+    shard_ranker = None  # shard_rank.ShardRanker of a model whose user_emb is this rank's block of a sharded table
+
     def __init__(self, conf, training_set, test_set, **kwargs):
         super(GraphRecommender, self).__init__(conf, training_set, test_set, **kwargs)
         self.data = Interaction(conf, training_set, test_set)
@@ -60,6 +63,9 @@ class GraphRecommender(Recommender):
         data = self.data
         names = list(data.test_set) if users is None else list(users)
         uids = np.fromiter((data.user[u] for u in names), dtype=np.int32, count=len(names))
+        if self.shard_ranker is not None:
+            ids, scores = self.shard_ranker.topk(self.user_emb.detach(), self.item_emb.detach(), uids, self.max_N)
+            return names, ids.cpu().numpy(), scores.cpu().numpy()
         rated_ptr, rated_idx = data.rated_csr()
         if self._has_embedding_tables():
             ids, scores = ops.score_topk(self.user_emb.detach(), self.item_emb.detach(), uids, rated_ptr, rated_idx, self.max_N)
@@ -99,13 +105,16 @@ class GraphRecommender(Recommender):
         stamp = strftime("%Y-%m-%d %H-%M-%S", localtime(time()))
         out_dir = self.output
         name = self.config["model"]["name"]
-        FileIO.write_file(out_dir, f"{name}@{stamp}-top-{self.max_N}items.txt", self.recOutput)
-        print("The result has been output to ", abspath(out_dir), ".")
+        main = is_main_process()  # every rank holds the same rec_list: one set of result files
+        if main:
+            FileIO.write_file(out_dir, f"{name}@{stamp}-top-{self.max_N}items.txt", self.recOutput)
+            print("The result has been output to ", abspath(out_dir), ".")
         self.result = ranking_evaluation(self.data.test_set, rec_list, self.topN)
         self.model_log.add("###Evaluation Results###")
         self.model_log.add(self.result)
-        FileIO.write_file(out_dir, f"{name}@{stamp}-performance.txt", self.result)
-        print(f"The result of {self.model_name}:\n{''.join(self.result)}")
+        if main:
+            FileIO.write_file(out_dir, f"{name}@{stamp}-performance.txt", self.result)
+            print(f"The result of {self.model_name}:\n{''.join(self.result)}")
 
     def _fast_measure(self):
         """fast_evaluation's metrics without leaving id space: full-catalog top-k on the device, hit masks on
@@ -113,13 +122,17 @@ class GraphRecommender(Recommender):
         ranking_evaluation(self.data.test_set, self.test(), [self.max_N])."""
         data = self.data
         names = list(data.test_set)
-        if not (self._has_embedding_tables() and self.max_N <= 64 and all(u in data.user for u in names)):
+        ranker = self.shard_ranker
+        if not ((ranker is not None or self._has_embedding_tables()) and self.max_N <= 64 and all(u in data.user for u in names)):
             return ranking_evaluation(data.test_set, self.test(), [self.max_N])
         uids = np.fromiter((data.user[u] for u in names), dtype=np.int32, count=len(names))
-        rated_ptr, rated_idx = data.rated_csr()
-        ids, _ = ops.score_topk(self.user_emb.detach(), self.item_emb.detach(), uids, rated_ptr, rated_idx, self.max_N)
         test_ptr, test_idx, n_test = data.test_csr()
-        masks = ops.rank_hit_masks(ids, uids, test_ptr, test_idx).cpu().numpy()
+        if ranker is not None:
+            masks = ranker.hit_masks(self.user_emb.detach(), self.item_emb.detach(), uids, self.max_N).cpu().numpy()
+        else:
+            rated_ptr, rated_idx = data.rated_csr()
+            ids, _ = ops.score_topk(self.user_emb.detach(), self.item_emb.detach(), uids, rated_ptr, rated_idx, self.max_N)
+            masks = ops.rank_hit_masks(ids, uids, test_ptr, test_idx).cpu().numpy()
         return ranking_evaluation_from_masks(n_test[uids], masks.view(np.uint64), [self.max_N])
 
     def fast_evaluation(self, epoch):
@@ -135,9 +148,10 @@ class GraphRecommender(Recommender):
         else:
             self.bestPerformance = [epoch + 1, performance]
             self.save()
-        print("-" * 80)
-        print(f"Real-Time Ranking Performance (Top-{self.max_N} Item Recommendation)")
-        print(f"*Current Performance*\nEpoch: {epoch + 1}, " + ", ".join(f"{k}: {v}" for k, v in performance.items()))
-        print(f"*Best Performance*\nEpoch: {self.bestPerformance[0]}, " + ", ".join(f"{k}: {v}" for k, v in self.bestPerformance[1].items()))
-        print("-" * 80)
+        if is_main_process():
+            print("-" * 80)
+            print(f"Real-Time Ranking Performance (Top-{self.max_N} Item Recommendation)")
+            print(f"*Current Performance*\nEpoch: {epoch + 1}, " + ", ".join(f"{k}: {v}" for k, v in performance.items()))
+            print(f"*Best Performance*\nEpoch: {self.bestPerformance[0]}, " + ", ".join(f"{k}: {v}" for k, v in self.bestPerformance[1].items()))
+            print("-" * 80)
         return measure

@@ -6,6 +6,7 @@ import os
 import time
 
 from ..data.data import Data
+from ..shard_rank import is_main_process
 from ..util.logger import Log
 
 # attribute, YAML key, conversion, label printed by print_model_info (None: not printed)
@@ -33,7 +34,7 @@ class Recommender:
         for attr, key, cast, _label in _SETTINGS:
             setattr(self, attr, cast(conf[key]))
         now = time.strftime("%Y-%m-%d %H-%M-%S", time.localtime(time.time()))
-        self.model_log = Log(self.model_name, self.model_name + " " + now)
+        self.model_log = Log(self.model_name, self.model_name + " " + now, to_file=is_main_process())
         self.result, self.recOutput = [], []
 
     def initializing_log(self):

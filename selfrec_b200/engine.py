@@ -82,7 +82,87 @@ def capture_step(enqueue, state, warm, warmups, barrier=lambda: None):
     return g
 
 
-class TrainEngine:
+def initial_tables(n_users, n_items, out):
+    """The reference's initial tables, drawn into `out` [U+I, d] (any device) from torch's global state: CPU
+    xavier_uniform_ users then items, the same initialiser calls in the same order as LightGCN.py:60-66; above 2^27
+    elements (config-5 sized tables, where a 6 GB host tensor is not worth its copy) xavier-uniform drawn on out's
+    device from a generator keyed by torch.initial_seed().  Returns (out[:U], out[U:])."""
+    U, N, d = int(n_users), int(n_users) + int(n_items), out.shape[1]
+    if N * d > (1 << 27):
+        g = torch.Generator(device=out.device).manual_seed(torch.initial_seed() & 0x7FFFFFFF)
+        for lo, hi in ((0, U), (U, N)):
+            bound = (6.0 / ((hi - lo) + d)) ** 0.5
+            out[lo:hi].uniform_(-bound, bound, generator=g)
+    else:
+        out[:U].copy_(torch.nn.init.xavier_uniform_(torch.empty(U, d)))
+        out[U:].copy_(torch.nn.init.xavier_uniform_(torch.empty(N - U, d)))
+    return out[:U], out[U:]
+
+
+class HostFeed:
+    """Host side of a training engine, shared by TrainEngine and the sharded engine: the epoch's batch words from the
+    native sampler, their copy through a ring of pinned slots into `batch_dev`, and the pinned D2H copy of `losses`.
+    The engine sets data, B, words, batch_dev and losses, then calls _init_feed()."""
+
+    def _init_feed(self):
+        self.ring = [torch.zeros(self.words, dtype=torch.int32).pin_memory() for _ in range(8)]
+        self.ring_ev = [None] * len(self.ring)
+        self.ring_pos = 0
+        self.loss_ring = [torch.zeros(4, dtype=torch.float32).pin_memory() for _ in range(8)]
+        self.loss_pos = 0
+        self.sampler = None
+
+    def _feed(self, batch_words):
+        """Enqueue the H2D copy of one batch through the next pinned slot."""
+        slot = self.ring_pos
+        self.ring_pos = (slot + 1) % len(self.ring)
+        ev = self.ring_ev[slot]
+        if ev is not None:
+            ev.synchronize()  # the copy that last used this pinned slot has finished
+        pin = self.ring[slot]
+        if isinstance(batch_words, torch.Tensor):
+            pin.copy_(batch_words)
+        else:
+            pin.numpy()[:] = batch_words
+        self.batch_dev.copy_(pin, non_blocking=True)
+        ev = torch.cuda.Event()
+        ev.record()
+        self.ring_ev[slot] = ev
+
+    def _fetch_loss(self):
+        """Enqueue the D2H copy of the four loss values; returns a LossHandle."""
+        ls = self.loss_pos
+        self.loss_pos = (ls + 1) % len(self.loss_ring)
+        self.loss_ring[ls].copy_(self.losses, non_blocking=True)
+        lev = torch.cuda.Event()
+        lev.record()
+        return LossHandle(self.loss_ring[ls], lev)
+
+    def batches(self, exact_lazy=False):
+        """One epoch of batch words from the native sampler (advances Python's `random`).  The yielded buffer is
+        reused: consume it (step() copies it into a pinned slot) before asking for the next one.  exact_lazy=True
+        hands Python's `random` state back after every batch, like the reference's generator would."""
+        if self.sampler is None:
+            self.sampler = NativePairSampler(self.data)
+        s = self.sampler
+        if not exact_lazy:
+            yield from stream_epoch(s, self.data, self.B, self.B)
+            return
+        s.pull_state()
+        perm = s.begin_epoch(want_perm=True)
+        permute_training_data(self.data, perm)
+        s.push_state()
+        buf = np.empty(self.words, dtype=np.int32)
+        while True:
+            s.pull_state()
+            b = s.next_batch(self.B, self.B, buf)
+            s.push_state()
+            if b == 0:
+                return
+            yield buf
+
+
+class TrainEngine(HostFeed):
     def __init__(self, model, data, emb_size, n_layers, batch_size, lr, reg, *, eps=0.0, tau=0.2, cl_rate=0.0,
                  layer_cl=0, l2_div=1.0, device=None, init_user=None, init_item=None, philox_seed=0x5EED):
         lib = _lib.require_device()
@@ -104,16 +184,9 @@ class TrainEngine:
         self.dev = torch.device("cuda", torch.cuda.current_device()) if device is None else torch.device(device)
         dev = self.dev
         self.params = torch.empty((self.N, self.d), device=dev, dtype=torch.float32)
-        if init_user is None and self.N * self.d > (1 << 27):
-            # config-5 sized tables: xavier-uniform drawn on the device (a 6 GB host tensor is not worth its copy)
-            g = torch.Generator(device=dev).manual_seed(torch.initial_seed() & 0x7FFFFFFF)
-            for lo, hi in ((0, self.U), (self.U, self.N)):
-                bound = (6.0 / ((hi - lo) + self.d)) ** 0.5
-                self.params[lo:hi].uniform_(-bound, bound, generator=g)
+        if init_user is None:
+            initial_tables(self.U, self.I, self.params)
         else:
-            if init_user is None:  # same initialiser calls, same order as LightGCN.py:60-66
-                init_user = torch.nn.init.xavier_uniform_(torch.empty(self.U, self.d))
-                init_item = torch.nn.init.xavier_uniform_(torch.empty(self.I, self.d))
             self.params[: self.U].copy_(init_user)
             self.params[self.U:].copy_(init_item)
         self.m = torch.zeros_like(self.params)
@@ -123,11 +196,7 @@ class TrainEngine:
         self.losses = torch.zeros(4, device=dev, dtype=torch.float32)
         self.words = _lib.BATCH_HEADER + 5 * self.B
         self.batch_dev = torch.zeros(self.words, device=dev, dtype=torch.int32)
-        self.ring = [torch.zeros(self.words, dtype=torch.int32).pin_memory() for _ in range(8)]
-        self.ring_ev = [None] * len(self.ring)
-        self.ring_pos = 0
-        self.loss_ring = [torch.zeros(4, dtype=torch.float32).pin_memory() for _ in range(8)]
-        self.loss_pos = 0
+        self._init_feed()
         self.adj = None
         if model != "MF":
             na = data.norm_adj
@@ -149,7 +218,6 @@ class TrainEngine:
         self._fork_stream, self._fork_events = fork_resources(s, self.dev)  # BPR beside InfoNCE
         self.desc = s
         self.eps, self.layer_cl = float(eps), int(layer_cl)
-        self.sampler = None
         self.graph = None
         self._warm = False
 
@@ -191,32 +259,12 @@ class TrainEngine:
         returns without synchronising.  fetch_loss=True also enqueues a D2H copy of the four loss
         values into pinned memory and returns a LossHandle; .get() waits for that copy only, so the
         caller can sample the next batch while this step runs."""
-        slot = self.ring_pos
-        self.ring_pos = (slot + 1) % len(self.ring)
-        ev = self.ring_ev[slot]
-        if ev is not None:
-            ev.synchronize()  # the copy that last used this pinned slot has finished
-        pin = self.ring[slot]
-        if isinstance(batch_words, torch.Tensor):
-            pin.copy_(batch_words)
-        else:
-            pin.numpy()[:] = batch_words
-        self.batch_dev.copy_(pin, non_blocking=True)
-        ev = torch.cuda.Event()
-        ev.record()
-        self.ring_ev[slot] = ev
+        self._feed(batch_words)
         if self.graph is not None:
             self.graph.replay()
         else:
             self._enqueue()
-        if not fetch_loss:
-            return None
-        ls = self.loss_pos
-        self.loss_pos = (ls + 1) % len(self.loss_ring)
-        self.loss_ring[ls].copy_(self.losses, non_blocking=True)
-        lev = torch.cuda.Event()
-        lev.record()
-        return LossHandle(self.loss_ring[ls], lev)
+        return self._fetch_loss() if fetch_loss else None
 
     def step_resident(self):
         """Step on whatever batch_dev currently holds (inputs already in HBM)."""
@@ -227,29 +275,6 @@ class TrainEngine:
         self.graph = capture_step(self._enqueue, (self.params, self.m, self.v, self.step_dev, self.losses), self._warm, 2)
         self._warm = True
         return self.graph
-
-    def batches(self, exact_lazy=False):
-        """One epoch of batch words from the native sampler (advances Python's `random`).  The yielded buffer is
-        reused: consume it (step() copies it into a pinned slot) before asking for the next one.  exact_lazy=True
-        hands Python's `random` state back after every batch, like the reference's generator would."""
-        if self.sampler is None:
-            self.sampler = NativePairSampler(self.data)
-        s = self.sampler
-        if not exact_lazy:
-            yield from stream_epoch(s, self.data, self.B, self.B)
-            return
-        s.pull_state()
-        perm = s.begin_epoch(want_perm=True)
-        permute_training_data(self.data, perm)
-        s.push_state()
-        buf = np.empty(self.words, dtype=np.int32)
-        while True:
-            s.pull_state()
-            b = s.next_batch(self.B, self.B, buf)
-            s.push_state()
-            if b == 0:
-                return
-            yield buf
 
     # ---- inference ---------------------------------------------------------------------
     def forward_clean(self):

@@ -2,12 +2,18 @@
 
 Each model keeps the reference class name, constructor signature, YAML keys, attributes
 (`model.embedding_dict`, `user_emb`, `item_emb`, `best_user_emb`, ...) and train()/save()/
-predict() contract; the batch loop body is one TrainEngine.step()."""
+predict() contract; the batch loop body is one engine step().
+
+Inside a process group (install() starts one under torchrun) the propagating models train on the bipartite-sharded
+engine, at any world size including 1: each rank holds its own users' rows, `best_user_emb` is that [Ug, d] block,
+and ranking goes through shard_rank.ShardRanker.  MF has no propagation to shard and keeps TrainEngine at world 1."""
 import torch
 import torch.nn as nn
 
+from ... import shard_rank
+from ..._lib import SrbError
 from ...base.graph_recommender import GraphRecommender
-from ...engine import TrainEngine
+from ...engine import TrainEngine, initial_tables
 
 
 class _EncoderView(nn.Module):
@@ -38,7 +44,24 @@ class FusedGraphModel(GraphRecommender):
         return {}
 
     def _make_engine(self, n_layers, **kw):
-        self.engine = TrainEngine(self.MODEL, self.data, self.emb_size, n_layers, self.batch_size, self.lRate, self.reg, **kw)
+        args = (self.MODEL, self.data, self.emb_size, n_layers, self.batch_size, self.lRate, self.reg)
+        pg = shard_rank.process_group()
+        if pg is not None:
+            rank, world = pg
+            if self.MODEL == "MF" and world > 1:
+                raise SrbError(f"MF has no propagation to shard: run it in one process, not on {world} ranks")
+            shard_rank.broadcast_start_state()  # one trajectory: rank 0's sampler stream, view draws and tables
+        if pg is None or self.MODEL == "MF":
+            self.engine = TrainEngine(*args, **kw)
+        else:
+            from ...sharded import ShardedEngine
+            dev = torch.device("cuda", torch.cuda.current_device())
+            n, d = int(self.data.user_num) + int(self.data.item_num), int(self.emb_size)
+            # the tables a single-process TrainEngine would draw; the engine keeps this rank's rows of them
+            init_user, init_item = initial_tables(self.data.user_num, self.data.item_num, torch.empty((n, d), device=dev))
+            self.engine = ShardedEngine(*args, init_user=init_user, init_item=init_item, device=dev, **kw)
+            del init_user, init_item
+            self.shard_ranker = shard_rank.ShardRanker(self.data, rank, world, dev)
         self.model = _EncoderView(self.engine)
 
     def _epoch_prologue(self, epoch):
@@ -55,7 +78,9 @@ class FusedGraphModel(GraphRecommender):
                 eng.capture()  # one CUDA graph launch per batch from here on
             for n, words in enumerate(eng.batches()):
                 if n % 100 == 0 and n > 0:
-                    self._log_line(epoch, n, eng.step(words, fetch_loss=True).get().tolist())
+                    losses = eng.step(words, fetch_loss=True).get().tolist()
+                    if shard_rank.is_main_process():  # the losses are replicated over the ranks
+                        self._log_line(epoch, n, losses)
                 else:
                     eng.step(words)
             with torch.no_grad():
@@ -70,7 +95,12 @@ class FusedGraphModel(GraphRecommender):
             self.best_user_emb, self.best_item_emb = ue.clone(), ie.clone()
 
     def predict(self, u):
-        u = self.data.get_user_id(u)
+        name, u = u, self.data.get_user_id(u)
+        if self.shard_ranker is not None:  # this rank holds the rows of the users it owns only
+            r = self.shard_ranker
+            if r.owner(u) != r.rank:
+                raise SrbError(f"predict: user {name!r} is owned by rank {r.owner(u)}, this is rank {r.rank}")
+            u = r.local_row(u)
         # one user's full-catalog scores (reference predict(), e.g. XSimGCL.py:57-60); test()
         # never calls this -- it uses the fused scoring + top-k kernel.
         from ... import ops

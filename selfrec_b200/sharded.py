@@ -21,6 +21,7 @@ import os
 import numpy as np
 
 from . import _lib
+from .engine import HostFeed
 
 
 def local_user_count(n_users, rank, world):
@@ -31,6 +32,16 @@ def local_user_count(n_users, rank, world):
 def user_ids_of(n_users, rank, world):
     """Global ids of rank's users in local-row order (numpy int64)."""
     return np.arange(int(rank), int(n_users), int(world), dtype=np.int64)
+
+
+def owner_of(users, world):
+    """Rank owning each global user id (numpy int64)."""
+    return np.asarray(users, dtype=np.int64) % int(world)
+
+
+def local_row_of(users, world):
+    """Local row of each global user id on its owning rank (numpy int64)."""
+    return np.asarray(users, dtype=np.int64) // int(world)
 
 
 def item_bounds(n_items, world):
@@ -73,11 +84,12 @@ def extract_blocks(rowptr, colidx, vals, n_users, n_items, rank, world):
     return ru, rt
 
 
-class ShardedEngine:
+class ShardedEngine(HostFeed):
     """LightGCN / SimGCL / XSimGCL / SGL training on bipartite-sharded tables; world == 1 works without torch.distributed.
 
-    Same constructor surface as TrainEngine.  Every rank must feed the SAME batch buffer to step().  Parameters:
-    `user_emb` = this rank's users [Ug, d] (global ids `user_ids`: rank, rank + world, ...), `item_emb` = the full
+    Same constructor surface as TrainEngine, and the same batches() / step(words, fetch_loss=...) host feed.  Every rank
+    must feed the SAME batch buffer to step(): draw batches() from the same Python `random` state on every rank.
+    Parameters: `user_emb` = this rank's users [Ug, d] (global ids `user_ids`: rank, rank + world, ...), `item_emb` = the full
     replicated [I, d] item table.  The in-kernel Philox noise is keyed by global row ids, so a sharded run with the same
     philox_seed draws the noise the single-GPU TrainEngine draws.  SGL needs set_view_graphs() once per epoch."""
 
@@ -93,6 +105,7 @@ class ShardedEngine:
             raise _lib.SrbError(f"embedding.size {emb_size} is not supported by the CUDA path {ops._SUPPORTED_D}")
         self.torch, self.ops, self.lib = torch, ops, lib
         self.model_name = model
+        self.data = data
         self.dist = None
         self.group = None
         self.rank, self.world = 0, 1
@@ -181,6 +194,7 @@ class ShardedEngine:
         self.losses = torch.zeros(4, device=dev)
         self.words = _lib.BATCH_HEADER + 5 * self.B
         self.batch_dev = torch.zeros(self.words, dtype=torch.int32, device=dev)
+        self._init_feed()
         s = _lib.ShardDesc()
         fill_step_fields(s, model, self.U, self.I, self.d, self.L, self.B, lr=lr, reg=reg, eps=eps, tau=tau, cl_rate=cl_rate,
                          layer_cl=layer_cl, l2_div=l2_div, philox_seed=philox_seed)
@@ -269,13 +283,15 @@ class ShardedEngine:
     def _enqueue(self):
         _lib.check(self.lib.srb_shard_step(C.byref(self.desc), self.ops._stream()), "srb_shard_step")
 
-    def step(self, words=None, words_dev=None):
-        torch = self.torch
+    def step(self, words=None, words_dev=None, fetch_loss=False):
+        """One step on host batch words (copied through a pinned slot), on a device batch buffer, or on whatever
+        batch_dev holds.  fetch_loss=True returns a LossHandle, as TrainEngine.step does."""
         if words_dev is not None:
             self.batch_dev.copy_(words_dev, non_blocking=True)
         elif words is not None:
-            self.batch_dev.copy_(torch.as_tensor(np.asarray(words, dtype=np.int32)), non_blocking=True)
+            self._feed(words)
         self.step_resident()
+        return self._fetch_loss() if fetch_loss else None
 
     def step_resident(self):
         if self.graph is not None:

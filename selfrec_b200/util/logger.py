@@ -14,10 +14,11 @@ def _file_handler(filename):
 
 
 class Log(object):
-    def __init__(self, module, filename):
+    def __init__(self, module, filename, to_file=True):
         self.logger = logging.getLogger(module)
         self.logger.setLevel(logging.INFO)
-        self.logger.addHandler(_file_handler(filename))
+        if to_file:  # False on the ranks other than 0 of a multi-process run: one log file per run
+            self.logger.addHandler(_file_handler(filename))
 
     def add(self, text):
         self.logger.info(text)
