@@ -307,7 +307,8 @@ static Blocks blocks(const Ctx& c, int q) {
 }
 
 // SRB_SHARD_SYNC=barrier: separate barrier launches between the kernels of a layer instead of waits / signals folded
-// into them (measurement switch; both are kept parity-tested)
+// into them (measurement switch; both are parity-tested: the folded mode by the one-process-per-GPU checks, barrier mode
+// by tests/test_gpu_shard_loopback.py, whose ranks share one GPU -- the only mode that can, since no other kernel waits)
 static bool sync_in_kernels() {
   static const int mode = [] {
     const char* e = getenv("SRB_SHARD_SYNC");

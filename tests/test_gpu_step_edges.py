@@ -47,10 +47,10 @@ def _norm_adj(pu, pi, n_users, n_items):
 class _HubData:
     """What the engines read from an Interaction: sizes, the (user, item) pairs and the normalised adjacency."""
 
-    def __init__(self, pu, pi):
-        self.user_num, self.item_num = U, I
+    def __init__(self, pu, pi, n_users=U, n_items=I):
+        self.user_num, self.item_num = n_users, n_items
         self.pair_users, self.pair_items = pu, pi
-        self.norm_adj = _norm_adj(pu, pi, U, I)
+        self.norm_adj = _norm_adj(pu, pi, n_users, n_items)
         self.training_data = []
 
 
@@ -69,53 +69,47 @@ def _words(u, i, j, tail_u, tail_i):
     return w
 
 
-@pytest.fixture(scope="module")
-def hub():
-    """U x I bipartite graph, background user degree 3..9, with explicit rows at every class boundary: users of degree
-    4096 / 4097 (split rows of 2 and 3 chunks), 4095, 256 / 255, 128 / 127, 64 / 63 and items of degree 5000 / 4096.
-    Plus the poison batch and the five batches that follow it."""
-    import torch
-    from selfrec_b200 import _lib, ops
-    rng = np.random.default_rng(20261016)
-    plain_items = np.arange(3, I)
-    bg_items = np.concatenate([[0], plain_items])  # every item but the two hubs
+def make_hub_graph(n_users, n_items, hub_users, hub_items, seed):
+    """n_users x n_items bipartite graph, background user degree 3..9, with the users `hub_users` and the items
+    `hub_items` ({id: degree}; the items' neighbours drawn from the other users) at the given degrees.  Users 1..9 and
+    items 1, 2 must be among them: the batches below put them in the hub triples.  Returns dict(data, A, poison,
+    batches, views): the graph, the poison batch, the five batches that follow it and SGL's view graphs."""
+    from selfrec_b200 import ops
+    U, I = n_users, n_items  # (shadow the module's sizes: everything below is sized by the graph it builds)
+    rng = np.random.default_rng(seed)
+    bg_items = np.setdiff1d(np.arange(I), list(hub_items))  # every item but the hubs
     pu, pi = [], []
     for u in range(U):
-        k = HUB_USERS.get(u, int(rng.integers(3, 10)))
+        k = hub_users.get(u, int(rng.integers(3, 10)))
         pu.append(np.full(k, u))
         pi.append(rng.choice(bg_items, k, replace=False))
-    ordinary_users = np.setdiff1d(np.arange(U), list(HUB_USERS))
-    for it, k in HUB_ITEMS.items():
+    ordinary_users = np.setdiff1d(np.arange(U), list(hub_users))
+    for it, k in hub_items.items():
         pu.append(rng.choice(ordinary_users, k, replace=False))
         pi.append(np.full(k, it))
-    data = _HubData(np.concatenate(pu).astype(np.int32), np.concatenate(pi).astype(np.int32))
+    data = _HubData(np.concatenate(pu).astype(np.int32), np.concatenate(pi).astype(np.int32), U, I)
     A = data.norm_adj
     deg = np.diff(A.indptr)
     assert A.nnz == 2 * len(data.pair_users), "pairs are distinct"
-    for u, k in HUB_USERS.items():
+    for u, k in hub_users.items():
         assert deg[u] == k, (u, deg[u])
-    for it, k in HUB_ITEMS.items():
+    for it, k in hub_items.items():
         assert deg[U + it] == k, (it, deg[U + it])
-    special = set(HUB_USERS) | {U + it for it in HUB_ITEMS}
-    assert max(deg[r] for r in range(U + I) if r not in special) < ops.LONG_ROW_NNZ - 1
+    special = np.zeros(U + I, dtype=bool)
+    special[list(hub_users)] = True
+    special[[U + it for it in hub_items]] = True
+    assert deg[~special].max() < ops.LONG_ROW_NNZ - 1
     assert deg[0] < ops.LONG_ROW_NNZ and deg[U] < ops.LONG_ROW_NNZ
-    c = ops.classify_rows(torch.from_numpy(A.indptr.astype(np.int32)))
-    order = c["row_order"].numpy()
-    assert c["n_huge"] == 4 and set(order[:4]) == {1, 2, U + 1, U + 2}
-    assert c["n_vlong"] == 2 and set(order[4:6]) == {3, 4}
-    assert c["n_long"] == 4 and set(order[6:10]) == {5, 6, 7, 8}
-    assert c["n_work"] == 2 + 3 + 3 + 2 and deg[order[10]] < ops.LONG_ROW_NNZ  # user 9 (63) is in the lane-group class
-    assert _lib.HUB_MIN_NNZ == 4096 and _lib.HUB_CHUNK == 2048
 
     # disjoint pools of ordinary rows: batch 1, batch 2, tails only
     perm_u = rng.permutation(np.setdiff1d(ordinary_users, [0]))
     a_u, c_u, p_u = perm_u[:100], perm_u[100:117], perm_u[117:]
-    perm_i = rng.permutation(np.arange(3, I))
+    perm_i = rng.permutation(np.setdiff1d(bg_items, [0]))
     a_i, c_i, p_i = perm_i[:150], perm_i[150:184], perm_i[184:]
     # poison batch: user 0, item 0, every hub and boundary row and every row a later batch uses, then tail-only rows
-    users = np.concatenate([[0], list(HUB_USERS), a_u, c_u])
+    users = np.concatenate([[0], list(hub_users), a_u, c_u])
     users = rng.permutation(np.concatenate([users, p_u[:B - len(users)]]))
-    items = np.concatenate([[0], list(HUB_ITEMS), a_i, c_i])
+    items = np.concatenate([[0], list(hub_items), a_i, c_i])
     items = rng.permutation(np.concatenate([items, p_i[:2 * B - len(items)]]))
     poison = (users, items[:B], items[B:])
 
@@ -125,11 +119,12 @@ def hub():
         assert 0 in tail_u and 0 in tail_i
         return _words(u, i, j, rng.permutation(tail_u), rng.permutation(tail_i)), (np.asarray(u), np.asarray(i), np.asarray(j))
 
-    # 1. a full batch without user 0: hub users in a third of the triples, every boundary user, the degree-5000 item a
-    #    positive 60 times, the degree-4096 item a positive in 10 triples and a negative in 10 others
+    # 1. a full batch without user 0: hub users in a third of the triples, every boundary user, item 1 a positive 60
+    #    times, item 2 a positive in 10 triples and a negative in 10 others, every further hub item a negative once
+    more = np.array([it for it in hub_items if it not in (1, 2)], dtype=np.int64)
     u1 = np.concatenate([rng.choice([1, 2], 80), [3, 4, 5, 6, 7, 8, 9], rng.choice(a_u, B - 87)])
     i1 = np.concatenate([np.full(60, 1), np.full(10, 2), rng.choice(a_i, B - 70)])
-    j1 = np.concatenate([rng.choice(a_i, 100), np.full(10, 2), rng.choice(a_i, B - 110)])
+    j1 = np.concatenate([rng.choice(a_i, 100), np.full(10, 2), more, rng.choice(a_i, B - 110 - len(more))])
     sh = rng.permutation(B)
     # 2. 17 triples on rows disjoint from batch 1; 3. one triple on a hub user; 4. empty; 5. one hub triple B times
     batches = [batch(u1[sh], i1[sh], j1[sh]), batch(c_u, c_i[:17], c_i[17:]), batch([2], [1], [a_i[0]]), batch([], [], []),
@@ -137,8 +132,8 @@ def hub():
     assert batches[0][0][1] < B and len(set(batches[0][1][0]) & set(c_u)) == 0 and batches[2][0][1] == batches[2][0][2] == 1
     poison_words = _words(*poison, poison[0], poison[1])  # b = cap: no tails
 
-    # SGL's view graphs: edge dropout at rate 0.1, and node dropout at rate 0.1 that also removes the degree-4096 user and
-    # the degree-5000 item (their view rows are empty, while the batch-row lists still classify them as split rows)
+    # SGL's view graphs: edge dropout at rate 0.1, and node dropout at rate 0.1 that also removes user 1 and item 1 (in
+    # the graphs here: split rows; their view rows are empty, while the batch-row lists still classify them as split rows)
     def edge_views():
         return [_norm_adj(data.pair_users[k], data.pair_items[k], U, I) for k in (rng.random(len(data.pair_users)) >= 0.1 for _ in range(2))]
 
@@ -156,15 +151,35 @@ def hub():
     return dict(data=data, A=A, poison=poison_words, batches=batches, views=views)
 
 
+@pytest.fixture(scope="module")
+def hub():
+    """U x I graph with explicit rows at every class boundary: users of degree 4096 / 4097 (split rows of 2 and 3
+    chunks), 4095, 256 / 255, 128 / 127, 64 / 63 and items of degree 5000 / 4096."""
+    import torch
+    from selfrec_b200 import _lib, ops
+    h = make_hub_graph(U, I, HUB_USERS, HUB_ITEMS, 20261016)
+    A = h["A"]
+    deg = np.diff(A.indptr)
+    c = ops.classify_rows(torch.from_numpy(A.indptr.astype(np.int32)))
+    order = c["row_order"].numpy()
+    assert c["n_huge"] == 4 and set(order[:4]) == {1, 2, U + 1, U + 2}
+    assert c["n_vlong"] == 2 and set(order[4:6]) == {3, 4}
+    assert c["n_long"] == 4 and set(order[6:10]) == {5, 6, 7, 8}
+    assert c["n_work"] == 2 + 3 + 3 + 2 and deg[order[10]] < ops.LONG_ROW_NNZ  # user 9 (63) is in the lane-group class
+    assert _lib.HUB_MIN_NNZ == 4096 and _lib.HUB_CHUNK == 2048
+    return h
+
+
 def _has_nan(torch, buf):
     n = buf.numel() - buf.numel() % 4
     return bool(torch.isnan(buf[:n].view(torch.float32)).any())
 
 
-def _poison(torch, eng, words, state, params, capture=False):
+def _poison(torch, eng, words, state, params, capture=False, workspaces=None):
     """One step with NaN parameters on `words`, then `state` put back: every float table the step writes is NaN wherever
     that step wrote it.  capture=True poisons through capture()'s warm-up steps instead of an eager step (capture()
-    restores what it saved, the NaN parameters included)."""
+    restores what it saved, the NaN parameters included).  `eng` needs step(words); workspaces: the buffers that must
+    hold NaN afterwards (default: eng.workspace)."""
     saved = [t.clone() for t in state]
     for t in params:
         t.fill_(float("nan"))
@@ -177,7 +192,8 @@ def _poison(torch, eng, words, state, params, capture=False):
     for dst, src in zip(state, saved):
         dst.copy_(src)
     torch.cuda.synchronize()
-    assert _has_nan(torch, eng.workspace), "the poison step left no NaN in the workspace"
+    for k, ws in enumerate([eng.workspace] if workspaces is None else workspaces):
+        assert _has_nan(torch, ws), f"the poison step left no NaN in workspace {k}"
 
 
 def _unambiguous_noise(orc, A, E0, noise):
@@ -197,12 +213,16 @@ def _unambiguous_noise(orc, A, E0, noise):
     return noise
 
 
-def _run_sequence(torch, orc, hub, name, d, L, lcl, view_csr, run_step, read_state, noise_dev, tag):
-    """The batches after the poison step, each against the oracle, continuing from the device state every step."""
+def _run_sequence(torch, orc, hub, name, d, L, lcl, view_csr, run_step, read_state, noise_dev, tag, eps=EPS, kappa=KAPPA):
+    """The batches after the poison step, each against the oracle, continuing from the device state every step.
+    SimGCL / XSimGCL without noise_dev: the step's own noise at eps = 0, where the perturbation vanishes.  kappa: the
+    first-moment bar (KAPPA)."""
+    KAPPA = kappa
     rng = np.random.default_rng(d * 100 + L * 10 + lcl)
     A = hub["A"]
-    N = U + I
+    U, N = hub["data"].user_num, A.shape[0]
     views = 2 if name == "SimGCL" else 1
+    assert noise_dev is not None or eps == 0.0 or name not in ("SimGCL", "XSimGCL")
     p, m, v, _ = read_state()
     for step, (words, (u, i, j)) in enumerate(hub["batches"], start=1):
         b = len(u)
@@ -211,6 +231,8 @@ def _run_sequence(torch, orc, hub, name, d, L, lcl, view_csr, run_step, read_sta
         if noise_dev is not None:
             noise = _unambiguous_noise(orc, A, p, rng.random((views, L, N, d), dtype=np.float32))
             noise_dev.copy_(torch.from_numpy(noise))
+        elif name in ("SimGCL", "XSimGCL"):
+            noise = np.zeros((views, L, 1, 1))  # (eps = 0: any noise adds nothing)
         run_step(words)
         torch.cuda.synchronize()
         gp, gm, gv, los = read_state()
@@ -221,7 +243,7 @@ def _run_sequence(torch, orc, hub, name, d, L, lcl, view_csr, run_step, read_sta
         if b == 0:
             g = np.zeros((N, d))
         else:
-            ref = orc.train_step(name, A, p, U, u, i, j, n_layers=L, reg=REG, batch_size=B, eps=EPS, tau=TAU, cl_rate=CL_RATE,
+            ref = orc.train_step(name, A, p, U, u, i, j, n_layers=L, reg=REG, batch_size=B, eps=eps, tau=TAU, cl_rate=CL_RATE,
                                  layer_cl=lcl, noise=noise, view_csr=view_csr)
             g = ref["grad"]
             for k, key in ((0, "rec"), (1, "l2")):
