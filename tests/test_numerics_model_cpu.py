@@ -10,6 +10,7 @@
 """
 import numpy as np
 import pytest
+from philox_model import philox4x32_10 as _philox4x32_10
 
 
 def tf32_trunc(x):
@@ -149,21 +150,6 @@ def test_fixed_shift_logsumexp_model(tau):
     got = shift + np.log(l, dtype=np.float32)
     assert np.isfinite(got).all() and (l > 0).all()
     assert np.abs(got - ref).max() <= 4e-7 / tau + 1e-6
-
-
-def _philox4x32_10(ctr, key):
-    """Philox4x32-10 (Salmon et al. 2011) on uint32 arrays: the generator of csrc/common.cuh."""
-    M0, M1, W0, W1 = np.uint64(0xD2511F53), np.uint64(0xCD9E8D57), np.uint32(0x9E3779B9), np.uint32(0xBB67AE85)
-    c = [np.asarray(x, dtype=np.uint32) for x in ctr]
-    k0, k1 = np.uint32(key[0]), np.uint32(key[1])
-    for _ in range(10):
-        p0 = M0 * c[0].astype(np.uint64)
-        p1 = M1 * c[2].astype(np.uint64)
-        hi0, lo0 = (p0 >> np.uint64(32)).astype(np.uint32), p0.astype(np.uint32)
-        hi1, lo1 = (p1 >> np.uint64(32)).astype(np.uint32), p1.astype(np.uint32)
-        c = [hi1 ^ c[1] ^ k0, lo1, hi0 ^ c[3] ^ k1, lo0]
-        k0, k1 = np.uint32((int(k0) + int(W0)) & 0xFFFFFFFF), np.uint32((int(k1) + int(W1)) & 0xFFFFFFFF)
-    return np.stack(c, -1)
 
 
 def test_philox_counter_layout_keeps_view_and_step_streams_apart():
