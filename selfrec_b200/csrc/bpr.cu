@@ -211,7 +211,8 @@ int scatter_segments(float* dst, int d, const ScatterSegs& segs, cudaStream_t st
     case 32: SRB_SCATTER(32)
     case 64: SRB_SCATTER(64)
     case 128: SRB_SCATTER(128)
-    default: set_error("scatter: unsupported d=%d (32, 64, 128)", d); return SRB_ERR_ARG;
+    case 256: SRB_SCATTER(256)
+    default: set_error("scatter: unsupported d=%d (32, 64, 128, 256)", d); return SRB_ERR_ARG;
   }
 #undef SRB_SCATTER
 }
@@ -337,8 +338,9 @@ extern "C" int srb_bpr_l2_fwd_bwd(const srb_bpr_desc* d, void* stream) {
     SRB_CASE(32)
     SRB_CASE(64)
     SRB_CASE(128)
+    SRB_CASE(256)
 #undef SRB_CASE
-    default: srb::set_error("bpr: unsupported d=%d (32, 64, 128)", d->d); return SRB_ERR_ARG;
+    default: srb::set_error("bpr: unsupported d=%d (32, 64, 128, 256)", d->d); return SRB_ERR_ARG;
   }
 }
 

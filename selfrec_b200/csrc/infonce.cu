@@ -12,6 +12,7 @@
 //   grad    per (row block, column split): G = (softmax(S) - I) * w/(n tau);
 //           dV1 += G V2 (registers, one atomic pass), dV2 += G^T V1 (red.v4 per tile)
 //                                                                            (6 n^2 d flop)
+//           (d = 256: nce_grad_wide_kernel, the column tile streamed in 128-wide halves)
 //   finish  back through F.normalize, loss = mean(lse - S_ii)
 #include "common.cuh"
 #include "infonce_tc.cuh"
@@ -450,6 +451,181 @@ __global__ void __launch_bounds__(256) nce_grad_kernel(const NceArgs a) {
   }
 }
 
+// D = 256: NceGradSmem<256> would take 288 KB, over the 227 KB a CTA may opt into.  The CTA's own 64 rows stay
+// resident (k-major and row-major, 128 KB) and every column tile is streamed in 128-wide halves: S accumulates over the
+// two k-halves of V2^T in the k order of s_tile (so S matches nce_lse_kernel<256> bit for bit), then G V2 and G^T V1
+// run over the two column halves of V2 and V1.  Per thread: o1 over both halves (2 x 4 x 8 registers), qv over one.
+constexpr int NCE_WIDE_D = 256;
+constexpr int NCE_WIDE_H = NCE_WIDE_D / 2;
+
+struct NceGradWideSmem {
+  float AsT[NCE_WIDE_D][NCE_T];  // own rows, k-major
+  float Ar[NCE_T][NCE_WIDE_D];   // own rows, row-major
+  float BsT[NCE_WIDE_H][NCE_T];  // one k-half of the column tile
+  float Br[NCE_T][NCE_WIDE_H];   // one column half of the column tile
+  float Gs[NCE_T][NCE_T];
+  float GsT[NCE_T][NCE_T];  // float4 column index xor-swizzled with (j >> 2), as in nce_grad_kernel
+  float lse[NCE_T];
+  float red[8];
+};
+
+__global__ void __launch_bounds__(256) nce_grad_wide_kernel(const NceArgs a) {
+  pdl_wait();
+  pdl_trigger();
+  constexpr int D = NCE_WIDE_D, H = NCE_WIDE_H;
+  constexpr int CW = H / 16;  // output columns per thread and half in the G V products
+  extern __shared__ __align__(16) unsigned char smem_raw[];
+  NceGradWideSmem& sm = *reinterpret_cast<NceGradWideSmem*>(smem_raw);
+  const NceProblem& p = a.p[blockIdx.z];
+  const int n = nce_n(p);
+  const int i0 = blockIdx.x * NCE_T;
+  if (i0 >= n) return;
+  const int split = blockIdx.y;
+  const int ty = threadIdx.x >> 4, tx = threadIdx.x & 15;
+  const float L2E = 1.4426950408889634f;
+  load_kmajor<D>(sm.AsT, p.V1T, a.np, i0);
+  load_rowmajor<D>(sm.Ar, p.V1, i0);
+  if (threadIdx.x < NCE_T) {
+    const int i = i0 + threadIdx.x;
+    float M = -INFINITY;
+    for (int s = 0; s < a.splits; ++s) M = fmaxf(M, p.part_m[(size_t)s * a.np + i]);
+    float Lsum = 0.f;
+    for (int s = 0; s < a.splits; ++s) {
+      const float ms = p.part_m[(size_t)s * a.np + i];
+      if (ms > -INFINITY) Lsum += p.part_l[(size_t)s * a.np + i] * exp2f((ms - M) * L2E);
+    }
+    const float lse = (i < n) ? M + logf(Lsum) : 0.f;
+    sm.lse[threadIdx.x] = lse;
+    float contrib = (split == 0 && i < n) ? lse - p.diag[i] : 0.f;
+    contrib = warp_sum(contrib);
+    if ((threadIdx.x & 31) == 0) sm.red[threadIdx.x >> 5] = contrib;
+  }
+  __syncthreads();
+  if (threadIdx.x == 0 && split == 0) atomicAdd(p.loss_acc, sm.red[0] + sm.red[1]);
+  const float gscale = p.weight * a.inv_tau / (float)n;
+  float o1[2][4][CW];
+#pragma unroll
+  for (int h = 0; h < 2; ++h)
+#pragma unroll
+    for (int r = 0; r < 4; ++r)
+#pragma unroll
+      for (int q = 0; q < CW; ++q) o1[h][r][q] = 0.f;
+  // one column half [h*H, h*H + H) of 64 row-major rows of V (row stride D)
+  auto load_half = [&](float (*dst)[H], const float* V, int row0, int h) {
+    for (int e = threadIdx.x; e < NCE_T * (H / 4); e += blockDim.x) {
+      const int r = e / (H / 4), c4 = e % (H / 4);
+      *reinterpret_cast<float4*>(&dst[r][c4 * 4]) = *reinterpret_cast<const float4*>(V + (size_t)(row0 + r) * D + h * H + c4 * 4);
+    }
+  };
+  const int ntiles = (n + NCE_T - 1) / NCE_T;
+  for (int jt = split; jt < ntiles; jt += a.splits) {
+    const int j0 = jt * NCE_T;
+    float s[4][4];
+#pragma unroll
+    for (int r = 0; r < 4; ++r)
+#pragma unroll
+      for (int c = 0; c < 4; ++c) s[r][c] = 0.f;
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      __syncthreads();  // h = 0: the previous tile's readers of BsT / Br / Gs are done; h = 1: the readers of k-half 0
+      load_kmajor<H>(sm.BsT, p.V2T + (size_t)h * H * a.np, a.np, j0);
+      if (h == 1) load_half(sm.Br, p.V2, j0, 0);
+      __syncthreads();
+#pragma unroll 8
+      for (int k = 0; k < H; ++k) {
+        const float4 av = *reinterpret_cast<const float4*>(&sm.AsT[h * H + k][ty * 4]);
+        const float4 bv = *reinterpret_cast<const float4*>(&sm.BsT[k][tx * 4]);
+        const float ar[4] = {av.x, av.y, av.z, av.w};
+        const float bc[4] = {bv.x, bv.y, bv.z, bv.w};
+#pragma unroll
+        for (int r = 0; r < 4; ++r)
+#pragma unroll
+          for (int c = 0; c < 4; ++c) s[r][c] = fmaf(ar[r], bc[c], s[r][c]);
+      }
+    }
+    // G = (exp(S - lse_i) - delta_ij) * gscale, zero outside the valid n x n block
+#pragma unroll
+    for (int r = 0; r < 4; ++r) {
+      const int i = i0 + ty * 4 + r;
+      const float lse = sm.lse[ty * 4 + r];
+#pragma unroll
+      for (int c = 0; c < 4; ++c) {
+        const int j = j0 + tx * 4 + c;
+        float g = 0.f;
+        if (i < n && j < n) {
+          g = exp2f((s[r][c] * a.inv_tau - lse) * L2E);
+          if (i == j) g -= 1.f;
+          g *= gscale;
+        }
+        s[r][c] = g;
+      }
+      *reinterpret_cast<float4*>(&sm.Gs[ty * 4 + r][tx * 4]) = make_float4(s[r][0], s[r][1], s[r][2], s[r][3]);
+    }
+#pragma unroll
+    for (int c = 0; c < 4; ++c) {
+      const int jl = tx * 4 + c;
+      *reinterpret_cast<float4*>(&sm.GsT[jl][((ty ^ (jl >> 2)) & 15) * 4]) = make_float4(s[0][c], s[1][c], s[2][c], s[3][c]);
+    }
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      if (h == 1) {
+        __syncthreads();  // the readers of column half 0 are done
+        load_half(sm.Br, p.V2, j0, 1);
+      }
+      __syncthreads();
+      // O1[i][h*H + c] += sum_j G[i][j] V2[j][h*H + c]
+#pragma unroll 4
+      for (int j = 0; j < NCE_T; ++j) {
+        const float4 av = *reinterpret_cast<const float4*>(&sm.GsT[j][((ty ^ (j >> 2)) & 15) * 4]);
+        const float ar[4] = {av.x, av.y, av.z, av.w};
+        float bq[CW];
+#pragma unroll
+        for (int q = 0; q < CW; ++q) bq[q] = sm.Br[j][tx * CW + q];
+#pragma unroll
+        for (int r = 0; r < 4; ++r)
+#pragma unroll
+          for (int q = 0; q < CW; ++q) o1[h][r][q] = fmaf(ar[r], bq[q], o1[h][r][q]);
+      }
+      // Q[j][h*H + c] = sum_i G[i][j] V1[i][h*H + c]
+      float qv[4][CW];
+#pragma unroll
+      for (int r = 0; r < 4; ++r)
+#pragma unroll
+        for (int q = 0; q < CW; ++q) qv[r][q] = 0.f;
+#pragma unroll 4
+      for (int i = 0; i < NCE_T; ++i) {
+        const float4 av = *reinterpret_cast<const float4*>(&sm.Gs[i][ty * 4]);
+        const float ar[4] = {av.x, av.y, av.z, av.w};
+        float bq[CW];
+#pragma unroll
+        for (int q = 0; q < CW; ++q) bq[q] = sm.Ar[i][h * H + tx * CW + q];
+#pragma unroll
+        for (int r = 0; r < 4; ++r)
+#pragma unroll
+          for (int q = 0; q < CW; ++q) qv[r][q] = fmaf(ar[r], bq[q], qv[r][q]);
+      }
+#pragma unroll
+      for (int r = 0; r < 4; ++r) {
+        const int j = j0 + ty * 4 + r;
+        if (j < n) {
+#pragma unroll
+          for (int q = 0; q < CW; ++q) atomicAdd(p.dV2 + (size_t)j * D + h * H + tx * CW + q, qv[r][q]);
+        }
+      }
+    }
+  }
+#pragma unroll
+  for (int r = 0; r < 4; ++r) {
+    const int i = i0 + ty * 4 + r;
+    if (i < n) {
+#pragma unroll
+      for (int h = 0; h < 2; ++h)
+#pragma unroll
+        for (int q = 0; q < CW; ++q) atomicAdd(p.dV1 + (size_t)i * D + h * H + tx * CW + q, o1[h][r][q]);
+    }
+  }
+}
+
 template <int D>
 __global__ void __launch_bounds__(256) nce_finish_kernel(const NceArgs a) {
   pdl_wait();
@@ -613,15 +789,24 @@ static int nce_launch(const NceArgs& a, int n_problems, cudaStream_t st) {
     SRB_TRY(launch_kernel(nce_prep_kernel<D>, grid, 256, 0, st, "nce_prep_kernel", a));
   }
   {
+    void (*grad)(const NceArgs);
+    size_t grad_smem;
+    if constexpr (D == NCE_WIDE_D) {
+      grad = nce_grad_wide_kernel;
+      grad_smem = sizeof(NceGradWideSmem);
+    } else {
+      grad = nce_grad_kernel<D>;
+      grad_smem = sizeof(NceGradSmem<D>);
+    }
     static bool attr_done = false;
     if (!attr_done) {
       SRB_TRY(check_cuda(cudaFuncSetAttribute(nce_lse_kernel<D>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(NceLseSmem<D>)), "nce lse smem attr"));
-      SRB_TRY(check_cuda(cudaFuncSetAttribute(nce_grad_kernel<D>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(NceGradSmem<D>)), "nce grad smem attr"));
+      SRB_TRY(check_cuda(cudaFuncSetAttribute(grad, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)grad_smem), "nce grad smem attr"));
       attr_done = true;
     }
     dim3 grid(np / NCE_T, a.splits, n_problems);
     SRB_TRY(launch_kernel(nce_lse_kernel<D>, grid, 256, sizeof(NceLseSmem<D>), st, "nce_lse_kernel", a));
-    SRB_TRY(launch_kernel(nce_grad_kernel<D>, grid, 256, sizeof(NceGradSmem<D>), st, "nce_grad_kernel", a));
+    SRB_TRY(launch_kernel(grad, grid, 256, grad_smem, st, D == NCE_WIDE_D ? "nce_grad_wide_kernel" : "nce_grad_kernel", a));
   }
   {
     dim3 grid((np + 7) / 8, n_problems);
@@ -641,7 +826,7 @@ extern "C" int srb_infonce_fwd_bwd(const srb_infonce_desc* d, void* stream) {
   SRB_REQUIRE(d != nullptr, "infonce: null desc");
   SRB_REQUIRE(d->n_problems >= 1 && d->n_problems <= 4, "infonce: n_problems must be 1..4");
   SRB_REQUIRE(d->temperature > 0.f, "infonce: temperature must be positive");
-  SRB_REQUIRE(d->d == 32 || d->d == 64 || d->d == 128, "infonce: unsupported d=%d (32, 64, 128)", d->d);
+  SRB_REQUIRE(d->d == 32 || d->d == 64 || d->d == 128 || d->d == 256, "infonce: unsupported d=%d (32, 64, 128, 256)", d->d);
   int max_n = 0;
   for (int q = 0; q < d->n_problems; ++q) {
     const srb_infonce_problem& s = d->prob[q];
@@ -710,6 +895,7 @@ extern "C" int srb_infonce_fwd_bwd(const srb_infonce_desc* d, void* stream) {
   switch (d->d) {
     case 32: return srb::nce_launch<32>(a, d->n_problems, st);
     case 64: return srb::nce_launch<64>(a, d->n_problems, st);
-    default: return srb::nce_launch<128>(a, d->n_problems, st);
+    case 128: return srb::nce_launch<128>(a, d->n_problems, st);
+    default: return srb::nce_launch<256>(a, d->n_problems, st);
   }
 }

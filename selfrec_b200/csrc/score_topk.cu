@@ -379,7 +379,8 @@ extern "C" int srb_score_topk(const srb_topk_desc* d, void* stream) {
     case 32: return srb::launch_topk<32>(a, (cudaStream_t)stream);
     case 64: return srb::launch_topk<64>(a, (cudaStream_t)stream);
     case 128: return srb::launch_topk<128>(a, (cudaStream_t)stream);
-    default: srb::set_error("topk: unsupported d=%d (32, 64, 128)", d->d); return SRB_ERR_ARG;
+    case 256: return srb::launch_topk<256>(a, (cudaStream_t)stream);  // 164 KB of shared memory (opt-in)
+    default: srb::set_error("topk: unsupported d=%d (32, 64, 128, 256)", d->d); return SRB_ERR_ARG;
   }
 }
 
@@ -404,7 +405,8 @@ extern "C" int srb_score_rows(const float* user_emb, const float* item_emb, int3
     case 32: srb::score_rows_kernel<32><<<grid, 256, 0, st>>>(user_emb, item_emb, users, n_items, out); break;
     case 64: srb::score_rows_kernel<64><<<grid, 256, 0, st>>>(user_emb, item_emb, users, n_items, out); break;
     case 128: srb::score_rows_kernel<128><<<grid, 256, 0, st>>>(user_emb, item_emb, users, n_items, out); break;
-    default: srb::set_error("score_rows: unsupported d=%d (32, 64, 128)", d); return SRB_ERR_ARG;
+    case 256: srb::score_rows_kernel<256><<<grid, 256, 0, st>>>(user_emb, item_emb, users, n_items, out); break;
+    default: srb::set_error("score_rows: unsupported d=%d (32, 64, 128, 256)", d); return SRB_ERR_ARG;
   }
   return srb::post_launch("score_rows_kernel");
 }

@@ -74,10 +74,14 @@ __device__ __forceinline__ void spmm_epilogue(const SpmmArgs& a, int row, int gl
       } else {
         const uint32_t stp = a.pstep ? (uint32_t)*a.pstep : 0u;
         const uint32_t grow = (uint32_t)(a.noise_row_base + row * a.noise_row_stride);
-        // counter = (row, column block | view << 16, layer tag, step): (view, step) pairs never share a stream
+        // counter = (row, column block | view << 16, layer tag, step): (view, step) pairs never share a stream; the
+        // column block (c / 4: gl and gl + LPR) stays below 64, clear of the view bits, up to D = 256
         const uint32_t vw = a.poff.y << 16;
-        const uint4 r0 = philox4x32_10(make_uint4(grow, (uint32_t)gl | vw, a.poff.x, stp), a.pkey);
-        const uint4 r1 = philox4x32_10(make_uint4(grow, (uint32_t)(gl + LPR) | vw, a.poff.x, stp), a.pkey);
+        const uint32_t cb0 = (uint32_t)gl | vw;
+        // (at LPR = 32, cb0 + 32: one add in place of a second loop-invariant word, which spilled at 64 registers)
+        const uint32_t cb1 = LPR == 32 ? cb0 + LPR : (uint32_t)(gl + LPR) | vw;
+        const uint4 r0 = philox4x32_10(make_uint4(grow, cb0, a.poff.x, stp), a.pkey);
+        const uint4 r1 = philox4x32_10(make_uint4(grow, cb1, a.poff.x, stp), a.pkey);
         n0 = make_float4(u32_to_unit(r0.x), u32_to_unit(r0.y), u32_to_unit(r0.z), u32_to_unit(r0.w));
         n1 = make_float4(u32_to_unit(r1.x), u32_to_unit(r1.y), u32_to_unit(r1.z), u32_to_unit(r1.w));
       }
@@ -158,15 +162,16 @@ __device__ __forceinline__ void spmm_epilogue(const SpmmArgs& a, int row, int gl
 }
 
 // Mapping: a row vector of D floats lives on LPR = D/8 lanes (two float4 per lane: columns
-// [4*gl, 4*gl+4) and [D/2 + 4*gl, ...)).  Rows are taken in `row_order` (degree-descending), in three
+// [4*gl, 4*gl+4) and [D/2 + 4*gl, ...)), so a warp holds 32/LPR lane groups: 8 at D = 32, one (the whole warp) at
+// D = 256.  Rows are taken in `row_order` (degree-descending), in three
 // classes so that no row is a long chain of dependent L2 round trips (a row of thousands of non-zeros handled by
 // one warp alone would take as long as the rest of the matrix):
-//   * the first n_vlong rows get a whole CTA: 8 warps x 4 lane groups stride through the row, partial
+//   * the first n_vlong rows get a whole CTA: 8 warps x 32/LPR lane groups stride through the row, partial
 //     sums meet in shared memory;
 //   * the next n_long rows get a warp each (the 32/LPR lane groups stride 32 non-zeros per iteration
-//     and are xor-shuffled together);
+//     and are xor-shuffled together; at D = 256 the warp is one group and there is nothing to combine);
 //   * the remaining rows are processed RPW = 32/LPR at a time, one per lane group (neighbours in the
-//     sorted order are equally long).
+//     sorted order are equally long; at D = 256 a warp per row).
 // Each lane loads one (col, val) pair per iteration (coalesced, prefetched one iteration ahead) and
 // the pairs are walked with group-wide shuffles; every X-row gather is two 128-bit ld.global.nc per
 // lane (LPR lanes x 16 B = one contiguous half row), issued 2*SB at a time before the FMAs.
@@ -224,7 +229,9 @@ __device__ __forceinline__ void spmm_gather(const SpmmArgs& a, int p, int end, i
       // group has run out -- fewer dependent L2 round trips, which is what bounds this product.  A slot past the
       // group's last hit loads nothing and adds an exact zero: X is a seed table whose rows outside the batch hold
       // whatever an earlier step left there (a NaN there would survive a multiplication by weight 0)
-      uint32_t gm = (__ballot_sync(SRB_FULL_MASK, hit) >> gbase) & ((1u << LPR) - 1u);
+      // (the group's LPR ballot bits; a whole-warp group at LPR = 32 keeps all of them -- 1u << 32 is undefined)
+      constexpr uint32_t GROUP_BITS = LPR >= 32 ? 0xffffffffu : (1u << (LPR & 31)) - 1u;
+      uint32_t gm = (__ballot_sync(SRB_FULL_MASK, hit) >> gbase) & GROUP_BITS;
       while (__any_sync(SRB_FULL_MASK, gm != 0)) {
         float vv[SB];
         float4 x0[SB], x1[SB];
@@ -254,6 +261,7 @@ __device__ __forceinline__ void spmm_gather(const SpmmArgs& a, int p, int end, i
   }
 }
 
+// sums the 32/lpr lane groups of a warp into every group (no shuffle at all when one group fills the warp)
 __device__ __forceinline__ void xor_reduce_groups(float4& acc0, float4& acc1, int lpr) {
   for (int o = lpr; o < 32; o <<= 1) {
     acc0.x += __shfl_xor_sync(SRB_FULL_MASK, acc0.x, o);
@@ -592,7 +600,8 @@ int launch_rows_epilogue(const SpmmArgs& a, int d, cudaStream_t st) {
     case 32: return launch_kernel(rows_epilogue_kernel<32>, (int)blocks, 256, 0, st, "rows_epilogue_kernel", a);
     case 64: return launch_kernel(rows_epilogue_kernel<64>, (int)blocks, 256, 0, st, "rows_epilogue_kernel", a);
     case 128: return launch_kernel(rows_epilogue_kernel<128>, (int)blocks, 256, 0, st, "rows_epilogue_kernel", a);
-    default: set_error("rows_epilogue: unsupported d=%d (32, 64, 128)", d); return SRB_ERR_ARG;
+    case 256: return launch_kernel(rows_epilogue_kernel<256>, (int)blocks, 256, 0, st, "rows_epilogue_kernel", a);
+    default: set_error("rows_epilogue: unsupported d=%d (32, 64, 128, 256)", d); return SRB_ERR_ARG;
   }
 }
 
@@ -607,7 +616,8 @@ int launch_reduce_rows(const SpmmArgs& a, const ReduceArgs& r, int d, cudaStream
     case 32: reduce_rows_kernel<32><<<(int)blocks, 256, 0, st>>>(a, r); break;
     case 64: reduce_rows_kernel<64><<<(int)blocks, 256, 0, st>>>(a, r); break;
     case 128: reduce_rows_kernel<128><<<(int)blocks, 256, 0, st>>>(a, r); break;
-    default: set_error("reduce_rows: unsupported d=%d (32, 64, 128)", d); return SRB_ERR_ARG;
+    case 256: reduce_rows_kernel<256><<<(int)blocks, 256, 0, st>>>(a, r); break;
+    default: set_error("reduce_rows: unsupported d=%d (32, 64, 128, 256)", d); return SRB_ERR_ARG;
   }
   return post_launch("reduce_rows_kernel");
 }
@@ -649,7 +659,8 @@ int launch_spmm(const SpmmArgs& a, int d, cudaStream_t st) {
     case 32: return launch_spmm_d<32>(a, (int)hub_blocks, (int)blocks, st);
     case 64: return launch_spmm_d<64>(a, (int)hub_blocks, (int)blocks, st);
     case 128: return launch_spmm_d<128>(a, (int)hub_blocks, (int)blocks, st);
-    default: set_error("spmm: unsupported d=%d (32, 64, 128)", d); return SRB_ERR_ARG;
+    case 256: return launch_spmm_d<256>(a, (int)hub_blocks, (int)blocks, st);
+    default: set_error("spmm: unsupported d=%d (32, 64, 128, 256)", d); return SRB_ERR_ARG;
   }
 }
 
