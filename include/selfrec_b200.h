@@ -543,6 +543,16 @@ int64_t srb_sampler_pairs(const srb_sampler* s);
 int srb_sampler_ring_start(srb_sampler* s, int32_t batch_size, int32_t batch_cap, int32_t depth);
 int srb_sampler_ring_pop(srb_sampler* s, int32_t* out);
 int srb_sampler_ring_stop(srb_sampler* s);
+/* Position, for checkpoints (refused while a ring runs: stop it first, which un-draws what was not popped).
+ * get/set_order: the current pair order (n_pairs users and items); set_order range-checks and copies.
+ * srb_sampler_cursor: *cursor = the pairs already consumed in the open epoch, -1 when no epoch is open.
+ * srb_sampler_seek: reopen an epoch at `cursor` (0..n_pairs) without shuffling, or close it (-1); with the order and
+ * the MT19937 state restored, the next batches -- sequential calls or a ring started now -- are the ones the
+ * uninterrupted epoch would have drawn. */
+int srb_sampler_get_order(const srb_sampler* s, int32_t* users, int32_t* items);
+int srb_sampler_set_order(srb_sampler* s, const int32_t* users, const int32_t* items, int64_t n_pairs);
+int srb_sampler_cursor(const srb_sampler* s, int64_t* cursor);
+int srb_sampler_seek(srb_sampler* s, int64_t cursor);
 
 /* ---------------------------------------------------------------------------------------
  * Bipartite-sharded training step (SURVEY 8e; selfrec_b200/csrc/sharded.cu).  One process per GPU.

@@ -190,6 +190,10 @@ SYMBOLS = {
     "srb_sampler_ring_start": (C.c_int, [VP, C.c_int32, C.c_int32, C.c_int32]),
     "srb_sampler_ring_pop": (C.c_int, [VP, c_i32p]),
     "srb_sampler_ring_stop": (C.c_int, [VP]),
+    "srb_sampler_get_order": (C.c_int, [VP, c_i32p, c_i32p]),
+    "srb_sampler_set_order": (C.c_int, [VP, c_i32p, c_i32p, C.c_int64]),
+    "srb_sampler_cursor": (C.c_int, [VP, c_i64p]),
+    "srb_sampler_seek": (C.c_int, [VP, C.c_int64]),
     "srb_shard_plan": (C.c_int, [C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32,
                                  C.POINTER(ShardLayout)]),
     "srb_shard_step": (C.c_int, [C.POINTER(ShardDesc), VP]),

@@ -189,6 +189,76 @@ extern "C" int srb_sampler_get_state(const srb_sampler* s, uint32_t* mt625) {
 
 extern "C" int64_t srb_sampler_pairs(const srb_sampler* s) { return s ? (int64_t)s->pu.size() : -1; }
 
+// ---- position: the pair order and the epoch cursor (checkpoints) --------------------------------------------------
+extern "C" int srb_sampler_get_order(const srb_sampler* s, int32_t* users, int32_t* items) {
+  if (!s || !users || !items) {
+    srb::set_error("sampler_get_order: null");
+    return SRB_ERR_ARG;
+  }
+  if (s->ring_running) {
+    srb::set_error("sampler_get_order: a ring is running");
+    return SRB_ERR_STATE;
+  }
+  memcpy(users, s->pu.data(), s->pu.size() * sizeof(int32_t));
+  memcpy(items, s->pi.data(), s->pi.size() * sizeof(int32_t));
+  return SRB_OK;
+}
+
+extern "C" int srb_sampler_set_order(srb_sampler* s, const int32_t* users, const int32_t* items, int64_t n_pairs) {
+  if (!s || !users || !items) {
+    srb::set_error("sampler_set_order: null");
+    return SRB_ERR_ARG;
+  }
+  if (s->ring_running) {
+    srb::set_error("sampler_set_order: a ring is running");
+    return SRB_ERR_STATE;
+  }
+  if (n_pairs != (int64_t)s->pu.size()) {
+    srb::set_error("sampler_set_order: %lld pairs, the sampler has %lld", (long long)n_pairs, (long long)s->pu.size());
+    return SRB_ERR_ARG;
+  }
+  for (int64_t t = 0; t < n_pairs; ++t) {
+    if (users[t] < 0 || users[t] >= s->n_users || items[t] < 0 || items[t] >= s->n_items) {
+      srb::set_error("sampler_set_order: pair %lld out of range", (long long)t);
+      return SRB_ERR_ARG;
+    }
+  }
+  memcpy(s->pu.data(), users, (size_t)n_pairs * sizeof(int32_t));
+  memcpy(s->pi.data(), items, (size_t)n_pairs * sizeof(int32_t));
+  return SRB_OK;
+}
+
+extern "C" int srb_sampler_cursor(const srb_sampler* s, int64_t* cursor) {
+  if (!s || !cursor) {
+    srb::set_error("sampler_cursor: null");
+    return SRB_ERR_ARG;
+  }
+  if (s->ring_running) {
+    srb::set_error("sampler_cursor: a ring is running");
+    return SRB_ERR_STATE;
+  }
+  *cursor = s->epoch_open ? s->ptr : -1;
+  return SRB_OK;
+}
+
+extern "C" int srb_sampler_seek(srb_sampler* s, int64_t cursor) {
+  if (!s) {
+    srb::set_error("sampler_seek: null");
+    return SRB_ERR_ARG;
+  }
+  if (s->ring_running) {
+    srb::set_error("sampler_seek: a ring is running");
+    return SRB_ERR_STATE;
+  }
+  if (cursor < -1 || cursor > (int64_t)s->pu.size()) {
+    srb::set_error("sampler_seek: cursor %lld outside -1..%lld", (long long)cursor, (long long)s->pu.size());
+    return SRB_ERR_ARG;
+  }
+  s->epoch_open = cursor >= 0;
+  s->ptr = cursor >= 0 ? cursor : 0;
+  return SRB_OK;
+}
+
 extern "C" int srb_sampler_begin_epoch(srb_sampler* s, int64_t* perm_out) {
   if (!s) {
     srb::set_error("sampler_begin_epoch: null");

@@ -9,12 +9,13 @@ import numpy as np
 class _PendingShuffles(object):
     """Epoch shuffles not yet applied to the list: new[k] = old[perm[k]], composed on demand."""
 
-    def __init__(self):
+    def __init__(self, fold=8):
         self.perms = []
+        self.fold = int(fold)
 
     def add(self, perm):
         self.perms.append(np.asarray(perm, dtype=np.int64))
-        if len(self.perms) >= 8:  # bound the memory: fold them into one permutation
+        if len(self.perms) >= self.fold:  # bound the memory: fold them into one permutation
             self.perms = [self.take()]
 
     def take(self):

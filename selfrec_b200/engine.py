@@ -82,6 +82,16 @@ def capture_step(enqueue, state, warm, warmups, barrier=lambda: None):
     return g
 
 
+def copy_rows_in(dst, src, what, chunk=1 << 20):
+    """dst [n, d] (device tensor, written in place) <- src [n, d] (numpy array or memmap), `chunk` rows at a time so a
+    memory-mapped source is never read into host memory whole."""
+    if tuple(src.shape) != tuple(dst.shape):
+        raise _lib.SrbError(f"load_state_dict: {what} is {tuple(src.shape)}, the engine's is {tuple(dst.shape)}")
+    for lo in range(0, dst.shape[0], chunk):
+        hi = min(dst.shape[0], lo + chunk)
+        dst[lo:hi].copy_(torch.from_numpy(np.require(src[lo:hi], np.float32, ["C", "W"])))  # a read-only map is copied
+
+
 def initial_tables(n_users, n_items, out):
     """The reference's initial tables, drawn into `out` [U+I, d] (any device) from torch's global state: CPU
     xavier_uniform_ users then items, the same initialiser calls in the same order as LightGCN.py:60-66; above 2^27
@@ -138,20 +148,43 @@ class HostFeed:
         lev.record()
         return LossHandle(self.loss_ring[ls], lev)
 
+    def _sampler(self):
+        if self.sampler is None:
+            self.sampler = NativePairSampler(self.data, track_order=getattr(self, "_track_order", False))
+        return self.sampler
+
+    def track_pair_order(self):
+        """Have the sampler keep the pair order as file positions, which feed_state() records (one n_pairs gather per
+        epoch; off by default).  Call it before the first epoch: an order shuffled untracked cannot be recovered."""
+        self._track_order = True
+        if self.sampler is not None:
+            self.sampler.track_order()
+
+    def feed_state(self):
+        """The sampler's position between two batches: {"order": int64 file positions of the pairs, "cursor": pairs
+        consumed in the open epoch (-1 between epochs), "random": Python's `random` state at that point}."""
+        order, cursor, st = self._sampler().position()
+        return {"order": order, "cursor": cursor, "random": st}
+
+    def load_feed_state(self, state):
+        """Restore feed_state(): the next batches() continues the saved epoch (or starts the next one)."""
+        self._sampler().restore(self.data, state["order"], state["cursor"], state["random"])
+
     def batches(self, exact_lazy=False):
         """One epoch of batch words from the native sampler (advances Python's `random`).  The yielded buffer is
         reused: consume it (step() copies it into a pinned slot) before asking for the next one.  exact_lazy=True
-        hands Python's `random` state back after every batch, like the reference's generator would."""
-        if self.sampler is None:
-            self.sampler = NativePairSampler(self.data)
-        s = self.sampler
+        hands Python's `random` state back after every batch, like the reference's generator would.  After
+        load_feed_state() of a mid-epoch position, the first call continues that epoch."""
+        s = self._sampler()
         if not exact_lazy:
             yield from stream_epoch(s, self.data, self.B, self.B)
             return
-        s.pull_state()
-        perm = s.begin_epoch(want_perm=True)
-        permute_training_data(self.data, perm)
-        s.push_state()
+        resume, s._resume = s._resume, False
+        if not resume:
+            s.pull_state()
+            perm = s.begin_epoch(want_perm=True)
+            permute_training_data(self.data, perm)
+            s.push_state()
         buf = np.empty(self.words, dtype=np.int32)
         while True:
             s.pull_state()
@@ -218,6 +251,8 @@ class TrainEngine(HostFeed):
         self._fork_stream, self._fork_events = fork_resources(s, self.dev)  # BPR beside InfoNCE
         self.desc = s
         self.eps, self.layer_cl = float(eps), int(layer_cl)
+        self.hyper = dict(lr=float(lr), reg=float(reg), eps=float(eps), tau=float(tau), cl_rate=float(cl_rate), layer_cl=int(layer_cl),
+                          l2_div=float(l2_div), philox_seed=int(philox_seed))
         self.graph = None
         self._warm = False
 
@@ -275,6 +310,32 @@ class TrainEngine(HostFeed):
         self.graph = capture_step(self._enqueue, (self.params, self.m, self.v, self.step_dev, self.losses), self._warm, 2)
         self._warm = True
         return self.graph
+
+    # ---- checkpoints ---------------------------------------------------------------------
+    def state_dict(self):
+        """The training state on the host, in the layout both engines share (checkpoint.py writes it):
+        step (the counter keying Adam's bias correction and the Philox stream), user_ids (global ids of the user rows,
+        here 0..U-1), user {params, m, v} [U, d], item_params [I, d], item_rows (the item rows whose moments this
+        engine owns: all of them) and item {m, v} of those rows.  Nothing else carries over from one step to the next:
+        the workspace, scalars and losses are rewritten by every step.  SGL's view graphs are the caller's (set_view_graphs)."""
+        U = self.U
+        return {"step": int(self.step_dev.item()), "user_ids": np.arange(U, dtype=np.int64),
+                "user": {"params": self.params[:U].cpu().numpy(), "m": self.m[:U].cpu().numpy(), "v": self.v[:U].cpu().numpy()},
+                "item_params": self.params[U:].cpu().numpy(), "item_rows": (0, self.I),
+                "item": {"m": self.m[U:].cpu().numpy(), "v": self.v[U:].cpu().numpy()}}
+
+    def load_state_dict(self, state):
+        """Copy a saved state into the engine's existing tensors (a captured CUDA graph stays valid: no address moves).
+        state: step, user {params, m, v} [U, d] in user id order, item_params [I, d], item {m, v} [I, d]; the arrays may
+        be memory maps (read in row chunks) and `user` / `item` any mapping that yields them on access."""
+        U = self.U
+        for name, dst in (("params", self.params), ("m", self.m), ("v", self.v)):
+            copy_rows_in(dst[:U], state["user"][name], "user " + name)
+        copy_rows_in(self.params[U:], state["item_params"], "item params")
+        for name, dst in (("m", self.m), ("v", self.v)):
+            copy_rows_in(dst[U:], state["item"][name], "item " + name)
+        self.step_dev.fill_(int(state["step"]))
+        torch.cuda.synchronize(self.dev)
 
     # ---- inference ---------------------------------------------------------------------
     def forward_clean(self):

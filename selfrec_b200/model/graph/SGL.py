@@ -4,6 +4,7 @@ Per epoch two augmented graphs (SGL.py:27-29, via GraphAugmentor + convert_to_la
 three encoders per step (clean + 2 views), one InfoNCE over cat(users, items) (SGL.py:120-125).
 The reference's `aug_type==0 or 1` test is always true (SGL.py:81), so every aug_type yields
 a single graph per view; that behaviour is kept."""
+from ..._lib import SrbError
 from ...data.augmentor import sample_range
 from ._common import FusedGraphModel
 
@@ -33,22 +34,59 @@ class SGL(FusedGraphModel):
         stream (GraphAugmentor's, natively: sample_range); only the kept positions travel to the GPU, where
         srb_graph_assemble builds D^-1/2 A D^-1/2 bit-identically to the scipy route (data/ui_graph.py:58-65,
         data/graph.py:10-24)."""
-        import torch
         bip = self._bipartite()
         if self.aug_type == 0:  # node dropout (augmentor.py:11-27): users first, then items, like the reference draws
             n_u, n_i = bip.U, bip.I
             du = sample_range(n_u, int(n_u * self.drop_rate))
             di = sample_range(n_i, int(n_i * self.drop_rate))
-            ku = torch.ones(n_u, dtype=torch.uint8, device=bip.dev)
-            ki = torch.ones(n_i, dtype=torch.uint8, device=bip.dev)
-            ku[torch.from_numpy(du).to(bip.dev)] = 0
-            ki[torch.from_numpy(di).to(bip.dev)] = 0
-            if getattr(self, "_ui_row", None) is None:
-                self._ui_row = torch.repeat_interleave(torch.arange(n_u, device=bip.dev), (bip.ui_ptr[1:] - bip.ui_ptr[:-1]).long())
-            flags = ku[self._ui_row] & ki[bip.ui_col.long()]
-            return bip.assemble(keep_flags=flags, reset_weights=True)
+            self._record(du, di)
+            return self._node_view(du, di)
         keep = sample_range(bip.nnz, int(bip.nnz * (1 - self.drop_rate)))  # edge dropout (augmentor.py:30-40)
+        self._record(keep)
         return bip.assemble(keep_idx=keep, reset_weights=True)
 
+    def _node_view(self, du, di):
+        """The view graph without the dropped users du and items di."""
+        import torch
+        bip = self._bipartite()
+        n_u, n_i = bip.U, bip.I
+        ku = torch.ones(n_u, dtype=torch.uint8, device=bip.dev)
+        ki = torch.ones(n_i, dtype=torch.uint8, device=bip.dev)
+        ku[torch.from_numpy(du).to(bip.dev)] = 0
+        ki[torch.from_numpy(di).to(bip.dev)] = 0
+        if getattr(self, "_ui_row", None) is None:
+            self._ui_row = torch.repeat_interleave(torch.arange(n_u, device=bip.dev), (bip.ui_ptr[1:] - bip.ui_ptr[:-1]).long())
+        flags = ku[self._ui_row] & ki[bip.ui_col.long()]
+        return bip.assemble(keep_flags=flags, reset_weights=True)
+
+    def _record(self, *draws):
+        if self._checkpoint_conf()["dir"] is not None:  # kept for a checkpoint inside the epoch
+            self.__dict__.setdefault("_draws", []).append(draws)
+
     def _epoch_prologue(self, epoch):
+        self._draws = []
         self.engine.set_view_graphs(self.random_graph_augment(), self.random_graph_augment())
+
+    # ---- checkpoints: the epoch's views travel as their draws, and are rebuilt bit for bit -------------------------
+    def _checkpoint_extra(self):
+        out = {}
+        for k, draws in enumerate(getattr(self, "_draws", [])):
+            for t, arr in enumerate(draws):
+                out[f"view{k}_draw{t}.npy"] = arr
+        return out
+
+    def _restore_extra(self, path):
+        import os
+        import numpy as np
+        views, restored = [], []
+        for k in range(2):
+            draws = []
+            while os.path.exists(os.path.join(path, f"view{k}_draw{len(draws)}.npy")):
+                draws.append(np.load(os.path.join(path, f"view{k}_draw{len(draws)}.npy")))
+            if len(draws) != (2 if self.aug_type == 0 else 1):
+                raise SrbError(f"checkpoint {path}: SGL view {k} has {len(draws)} draw files for aug_type {self.aug_type}")
+            views.append(self._node_view(*draws) if self.aug_type == 0 else
+                         self._bipartite().assemble(keep_idx=draws[0], reset_weights=True))
+            restored.append(tuple(draws))
+        self._draws = restored  # for a later save inside this epoch
+        self.engine.set_view_graphs(*views)

@@ -7,6 +7,9 @@ predict() contract; the batch loop body is one engine step().
 Inside a process group (install() starts one under torchrun) the propagating models train on the bipartite-sharded
 engine, at any world size including 1: each rank holds its own users' rows, `best_user_emb` is that [Ug, d] block,
 and ranking goes through shard_rank.ShardRanker.  MF has no propagation to shard and keeps TrainEngine at world 1."""
+import os
+
+import numpy as np
 import torch
 import torch.nn as nn
 
@@ -70,23 +73,115 @@ class FusedGraphModel(GraphRecommender):
     def _log_line(self, epoch, n, losses):
         print("training:", epoch + 1, "batch", n, "rec_loss:", losses[0], "cl_loss", losses[2])
 
+    # ---- checkpoints (optional YAML keys checkpoint.dir / checkpoint.every / checkpoint.resume) ------------------
+    def _checkpoint_conf(self):
+        if getattr(self, "_ckpt", None) is None:
+            conf = self.config
+            get = lambda key: conf[key] if conf.contain(key) else None
+            every = get("checkpoint.every")
+            self._ckpt = {"dir": get("checkpoint.dir"), "every": int(every) if every else 0, "resume": get("checkpoint.resume")}
+            if self._ckpt["every"] < 0:
+                raise SrbError(f"checkpoint.every must be a positive number of batches, not {every}")
+        return self._ckpt
+
+    def _fingerprint(self):
+        from ... import checkpoint
+        if getattr(self, "_pairs_fp", None) is None:
+            self._pairs_fp = checkpoint.pairs_fingerprint(self.data.pair_users, self.data.pair_items)
+        return self._pairs_fp
+
+    def _checkpoint_extra(self):
+        """{file name: array} of the model's own state inside an epoch (SGL: the draws of the epoch's views)."""
+        return {}
+
+    def _restore_extra(self, path):
+        pass
+
+    def _rank_world(self):
+        eng = self.engine
+        return (int(eng.rank), int(eng.world)) if hasattr(eng, "world") else (0, 1)
+
+    def save_checkpoint(self, epoch, batch):
+        """Write the run's state under checkpoint.dir: the engine, the sampler's position, the RNG states and the
+        keep-best tables, to continue at batch `batch` of epoch `epoch` (0-based).  Collective under a process group."""
+        from ... import checkpoint
+        eng = self.engine
+        rank, world = self._rank_world()
+        pos = eng.feed_state()  # first: the stream position, before anything else could draw
+        state = eng.state_dict()
+        man = checkpoint.identity(self.MODEL, eng, self.data, self._fingerprint())
+        bounds = [int(x) for x in eng.ib] if hasattr(eng, "ib") else [0, int(eng.I)]
+        man.update(epoch=int(epoch), batch=int(batch), step=state["step"], cursor=int(pos["cursor"]), item_bounds=bounds,
+                   bestPerformance=self.bestPerformance, rng=checkpoint.rng_states(pos["random"]))
+        common = {"item_params.npy": state["item_params"], "pair_order.npy": pos["order"]}
+        best_user = None
+        if getattr(self, "best_item_emb", None) is not None:
+            common["best_item.npy"] = self.best_item_emb.cpu().numpy()
+            best_user = self.best_user_emb.cpu().numpy()
+        if pos["cursor"] >= 0:
+            common.update(self._checkpoint_extra())
+        agree = eng.all_ok if world > 1 else (lambda ok: ok)
+        return checkpoint.save(self._checkpoint_conf()["dir"], man, {rank: (state, best_user)}, common, rank=rank, world=world,
+                               agree=agree)
+
+    def load(self, path=None):
+        """Restore a checkpoint (default: checkpoint.resume) into this model: the engine's tables, moments and step
+        counter, the sampler's order and position, the RNG states, the keep-best tables and bestPerformance.  train()
+        then continues at the saved epoch and batch.  A checkpoint of another model, shape, hyperparameter set or
+        training set is refused (SrbError) before anything is loaded."""
+        from ... import checkpoint
+        ck = self._checkpoint_conf()
+        path = checkpoint.resolve(ck["resume"] if path is None else path, ck["dir"])
+        man = checkpoint.read_manifest(path)
+        eng = self.engine
+        checkpoint.verify(man, checkpoint.identity(self.MODEL, eng, self.data, self._fingerprint()), path)
+        ids = checkpoint.engine_user_ids(eng)
+        eng.load_state_dict(checkpoint.engine_state(path, man, ids))
+        checkpoint.set_rng_states(man["rng"], python=False)
+        eng.load_feed_state({"order": np.load(os.path.join(path, "pair_order.npy")), "cursor": int(man["cursor"]),
+                             "random": checkpoint.python_random_state(man["rng"])})
+        self.bestPerformance = man["bestPerformance"]
+        if os.path.exists(os.path.join(path, "best_item.npy")):
+            dev = eng.dev
+            self.best_item_emb = torch.from_numpy(np.load(os.path.join(path, "best_item.npy"))).to(dev)
+            self.best_user_emb = torch.from_numpy(checkpoint.read_user_rows(path, man, "best", ids)).to(dev)
+        self._resume_at = (int(man["epoch"]), int(man["batch"]), int(man["cursor"]) >= 0)
+        if self._resume_at[2]:
+            self._restore_extra(path)
+        return path
+
+    def build(self):
+        if self._checkpoint_conf()["resume"] is not None:
+            self.load()
+
     def train(self):
         eng = self.engine
-        for epoch in range(self.maxEpoch):
-            self._epoch_prologue(epoch)
+        ck = self._checkpoint_conf()
+        every = ck["every"] if ck["dir"] is not None else 0
+        start_epoch, start_batch, mid_epoch = getattr(self, "_resume_at", (0, 0, False))
+        if ck["dir"] is not None:
+            eng.track_pair_order()  # the sampler keeps the pair order a checkpoint records (one gather per epoch)
+        for epoch in range(start_epoch, self.maxEpoch):
+            resumed = mid_epoch and epoch == start_epoch  # this epoch's prologue (SGL: its views) came with the checkpoint
+            if not resumed:
+                self._epoch_prologue(epoch)
             if eng.graph is None:
                 eng.capture()  # one CUDA graph launch per batch from here on
-            for n, words in enumerate(eng.batches()):
+            for n, words in enumerate(eng.batches(), start_batch if resumed else 0):
                 if n % 100 == 0 and n > 0:
                     losses = eng.step(words, fetch_loss=True).get().tolist()
                     if shard_rank.is_main_process():  # the losses are replicated over the ranks
                         self._log_line(epoch, n, losses)
                 else:
                     eng.step(words)
+                if every and (n + 1) % every == 0:
+                    self.save_checkpoint(epoch, n + 1)
             with torch.no_grad():
                 self.user_emb, self.item_emb = eng.forward_clean()
             if epoch >= self.EVAL_FROM and epoch % self.EVAL_EVERY == 0:
                 self.fast_evaluation(epoch)
+            if ck["dir"] is not None:
+                self.save_checkpoint(epoch + 1, 0)
         self.user_emb, self.item_emb = self.best_user_emb, self.best_item_emb
 
     def save(self):

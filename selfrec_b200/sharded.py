@@ -215,6 +215,8 @@ class ShardedEngine(HostFeed):
         s.nvls = 1 if (want_nvls and mc_ptr) else 0
         self.use_nvls = bool(s.nvls)
         self.desc = s
+        self.hyper = dict(lr=float(lr), reg=float(reg), eps=float(eps), tau=float(tau), cl_rate=float(cl_rate), layer_cl=int(layer_cl),
+                          l2_div=float(l2_div), philox_seed=int(philox_seed))
         self.view_blocks = None
         self.graph = None
         self._warm = False
@@ -265,6 +267,23 @@ class ShardedEngine(HostFeed):
         if self.dist is not None and self.world > 1:
             self.dist.barrier(self.group)
 
+    def _quiesce(self):
+        """Every rank's enqueued work finished, peer stores included: drain this device, then a host barrier (each rank
+        passes it only after its own device is drained, so every store a peer made into this rank's memory has landed)."""
+        self.torch.cuda.synchronize(self.dev)
+        self._host_barrier()
+
+    def all_ok(self, ok):
+        """True when `ok` is true on every rank (one all-reduce; a rank that failed tells the others instead of leaving
+        them in a barrier).  Collective."""
+        if self.dist is None or self.world == 1:
+            return bool(ok)
+        torch = self.torch
+        dev = self.dev if self.dist.get_backend(self.group) == "nccl" else "cpu"
+        t = torch.tensor([0 if ok else 1], dtype=torch.int32, device=dev)
+        self.dist.all_reduce(t, op=self.dist.ReduceOp.MAX, group=self.group)
+        return int(t.item()) == 0
+
     def check_peers(self):
         """Raise if a device-side barrier ever timed out (a peer died or fell out of step)."""
         if int(self._ctrl[1].item()) != 0:
@@ -306,6 +325,38 @@ class ShardedEngine(HostFeed):
         self.graph = capture_step(self._enqueue, state, self._warm, 1, self._host_barrier)
         self._warm = True
         return self.graph
+
+    # ---- checkpoints -----------------------------------------------------------------------
+    def state_dict(self):
+        """This rank's training state on the host, in TrainEngine.state_dict()'s layout: its users' rows (global ids
+        `user_ids`) of the parameters and moments, the replicated item table, and the item moments of the slice
+        [ib[rank], ib[rank + 1]) whose reduction it owns (only the owner updates those rows of mi / vi).
+
+        Collective.  A step returns without waiting for its peers: the owners' last item stores into this rank's copy of
+        the item table (the Adam epilogue of the owner-side reduction) may still be in flight when this rank's own stream
+        is done.  Every rank therefore drains its device and meets the others at a barrier before anything is read."""
+        self._quiesce()
+        lo, hi = int(self.ib[self.rank]), int(self.ib[self.rank + 1])
+        return {"step": int(self.step_dev.item()), "user_ids": self.user_ids.cpu().numpy().astype(np.int64),
+                "user": {"params": self.user_emb.cpu().numpy(), "m": self.mu.cpu().numpy(), "v": self.vu.cpu().numpy()},
+                "item_params": self.item_emb.cpu().numpy(), "item_rows": (lo, hi),
+                "item": {"m": self.mi[lo:hi].cpu().numpy(), "v": self.vi[lo:hi].cpu().numpy()}}
+
+    def load_state_dict(self, state):
+        """Copy a saved state into this rank's existing tensors (no address moves).  state: step, user {params, m, v}
+        [Ug, d] of this rank's users in local-row order, item_params [I, d] and item {m, v} [I, d] (every rank reads the
+        same item arrays, so the replicas stay bit-identical).  Collective: no peer's step may still be storing into
+        this rank's item table while it is overwritten (see state_dict())."""
+        from .engine import copy_rows_in
+        self._quiesce()
+        for name, dst in (("params", self.user_emb), ("m", self.mu), ("v", self.vu)):
+            copy_rows_in(dst, state["user"][name], "user " + name)
+        copy_rows_in(self.item_emb, state["item_params"], "item params")
+        for name, dst in (("m", self.mi), ("v", self.vi)):
+            copy_rows_in(dst, state["item"][name], "item " + name)
+        self.step_dev.fill_(int(state["step"]))
+        self.torch.cuda.synchronize(self.dev)
+        self._host_barrier()
 
     # ---- inference -------------------------------------------------------------------------
     def forward_clean(self):

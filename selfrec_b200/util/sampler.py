@@ -11,12 +11,13 @@ import random
 import numpy as np
 
 from .. import _lib
+from ..data.data import _PendingShuffles
 
 
 class NativePairSampler:
     """Owns a srb_sampler for one Interaction object."""
 
-    def __init__(self, data):
+    def __init__(self, data, track_order=False):
         lib = _lib.load()
         pu = np.ascontiguousarray(data.pair_users if hasattr(data, "pair_users") else [data.user[p[0]] for p in data.training_data], dtype=np.int32)
         pi = np.ascontiguousarray(data.pair_items if hasattr(data, "pair_items") else [data.item[p[1]] for p in data.training_data], dtype=np.int32)
@@ -27,6 +28,13 @@ class NativePairSampler:
         if not self.handle:
             raise _lib.SrbError("srb_sampler_create failed: " + _lib.last_error())
         self._state = (C.c_uint32 * 625)()
+        # the pair order as positions in the training file (new_order[k] = file index) while tracked: every epoch's
+        # permutation is composed into it (track_order; one n_pairs gather per epoch).  Nothing pending = the file
+        # order; None = unknown (an epoch was shuffled untracked)
+        self._tracking = bool(track_order)
+        self._shuffles = _PendingShuffles(fold=2)
+        self._ring = None     # (batch_size, batch_cap, depth) of the running ring
+        self._resume = False  # restore() reopened an epoch: the next stream_epoch continues it
 
     def __del__(self):
         if getattr(self, "handle", None):
@@ -47,7 +55,93 @@ class NativePairSampler:
         perm = np.empty(self.n_pairs, dtype=np.int64) if want_perm else None
         ptr = perm.ctypes.data_as(_lib.c_i64p) if want_perm else None
         _lib.check(self._lib.srb_sampler_begin_epoch(self.handle, ptr), "srb_sampler_begin_epoch")
+        if self._shuffles is not None:
+            if want_perm and self._tracking:
+                self._shuffles.add(perm)
+            else:
+                self._shuffles = None
         return perm
+
+    def track_order(self):
+        """Keep the pair order from here on (file_order()).  Only an order never shuffled untracked is known."""
+        self._tracking = True
+
+    # ---- position (checkpoints) ----------------------------------------------------------
+    def file_order(self):
+        """The current pair order as int64 positions in the training file (pair_users / pair_items order)."""
+        if self._shuffles is None:
+            raise _lib.SrbError("sampler: an epoch was shuffled while the pair order was not tracked; it is unknown (enable "
+                                "track_order before the first epoch: checkpoint.dir, or HostFeed.track_pair_order())")
+        order = self._shuffles.take()
+        order = np.arange(self.n_pairs, dtype=np.int64) if order is None else order
+        self._shuffles.add(order)
+        return order
+
+    def pair_order(self):
+        """(users, items) int32 in the sampler's current order (srb_sampler_get_order)."""
+        u, i = np.empty(self.n_pairs, dtype=np.int32), np.empty(self.n_pairs, dtype=np.int32)
+        ring = self._pause()
+        try:
+            _lib.check(self._lib.srb_sampler_get_order(self.handle, u.ctypes.data_as(_lib.c_i32p), i.ctypes.data_as(_lib.c_i32p)),
+                       "srb_sampler_get_order")
+        finally:
+            self._unpause(ring)
+        return u, i
+
+    def _pause(self):
+        ring = self._ring
+        if ring is not None:
+            self.ring_stop()  # un-draws what the consumer has not popped
+        return ring
+
+    def _unpause(self, ring):
+        if ring is not None:
+            self.ring_start(*ring)  # continues from the cursor
+
+    def position(self):
+        """(order, cursor, random_state) at the current batch boundary: the file order of the pairs, the pairs consumed
+        in the open epoch (-1 between epochs) and Python's `random` state at that point of the stream (inside an epoch
+        the stream lives in the sampler, not in `random`).  A running ring is paused for the read and restarted."""
+        ring = self._pause()
+        try:
+            cur = C.c_int64(0)
+            _lib.check(self._lib.srb_sampler_cursor(self.handle, C.byref(cur)), "srb_sampler_cursor")
+            cursor = int(cur.value)
+            if cursor >= 0:
+                _lib.check(self._lib.srb_sampler_get_state(self.handle, self._state), "srb_sampler_get_state")
+                st = (3, tuple(self._state), getattr(self, "_gauss", random.getstate()[2]))
+            else:
+                st = random.getstate()
+        finally:
+            self._unpause(ring)
+        return self.file_order(), cursor, st
+
+    def restore(self, data, order, cursor, random_state):
+        """Put the pairs in `order` (file positions, as position() returned them), reopen the epoch at `cursor` (-1:
+        between epochs) and set Python's `random` to `random_state`.  `data`'s training_data follows the order.  The
+        next stream_epoch() then continues the epoch instead of starting one."""
+        if getattr(self, "_open_epoch", None) is not None:  # an abandoned epoch generator: retire it (stream_epoch)
+            self._open_epoch, self._ring = None, None
+            self.ring_stop()
+        order = np.ascontiguousarray(order, dtype=np.int64)
+        if order.shape != (self.n_pairs,):
+            raise _lib.SrbError(f"sampler.restore: an order of {order.shape} for {self.n_pairs} pairs")
+        pu, pi = np.asarray(data.pair_users), np.asarray(data.pair_items)
+        u, i = np.ascontiguousarray(pu[order], dtype=np.int32), np.ascontiguousarray(pi[order], dtype=np.int32)
+        _lib.check(self._lib.srb_sampler_set_order(self.handle, u.ctypes.data_as(_lib.c_i32p), i.ctypes.data_as(_lib.c_i32p),
+                                                   self.n_pairs), "srb_sampler_set_order")
+        _lib.check(self._lib.srb_sampler_seek(self.handle, int(cursor)), "srb_sampler_seek")
+        # training_data is in the order this sampler's shuffles left it: move it from there to `order`
+        cur = self.file_order()
+        inv = np.empty_like(cur)
+        inv[cur] = np.arange(self.n_pairs, dtype=np.int64)
+        permute_training_data(data, inv[order])
+        self._shuffles = _PendingShuffles(fold=2)
+        self._shuffles.add(order)
+        self._tracking = True
+        self._resume = int(cursor) >= 0
+        random.setstate(random_state)
+        self.pull_state()  # the sampler's generator too: position() before the next batch reads it
 
     def next_batch_negs(self, batch_size, n_negs, u, i, j):
         b = self._lib.srb_sampler_next_batch_negs(self.handle, batch_size, n_negs, u.ctypes.data_as(_lib.c_i32p),
@@ -94,22 +188,27 @@ def stream_epoch(sampler, data, batch_size, batch_cap, ring_depth=16):
     queue hand-offs under the GIL cost more than they hid).  ring_depth=0: one native call per batch.  Python's
     `random` state is taken at the start and handed back when the epoch ends or the generator is closed (batches the
     ring sampled ahead but nobody read are un-drawn: the state is the reference's at that point of the stream);
-    data.training_data gets the epoch's shuffle."""
+    data.training_data gets the epoch's shuffle.  After sampler.restore() reopened an epoch, the generator continues
+    that epoch from its cursor instead (no shuffle); sampler.position() may be read between two batches."""
     # an epoch generator that was abandoned without close() (e.g. zip(range(n), gen)) still owns the ring and a
     # pending state hand-back: retire it now -- its own `finally`, whenever the garbage collector gets to it, must
     # neither stop the new ring nor overwrite Python's `random` state with a stale one
     if getattr(sampler, "_open_epoch", None) is not None:
+        sampler._ring = None
         sampler.ring_stop()
         sampler.push_state()
     token = object()
     sampler._open_epoch = token
+    resume, sampler._resume = getattr(sampler, "_resume", False), False
     sampler.pull_state()
     try:
-        perm = sampler.begin_epoch(want_perm=True)
-        permute_training_data(data, perm)
+        if not resume:
+            perm = sampler.begin_epoch(want_perm=True)
+            permute_training_data(data, perm)
         buf = np.empty(_lib.BATCH_HEADER + 5 * batch_cap, dtype=np.int32)
         if ring_depth > 0:
             sampler.ring_start(batch_size, batch_cap, ring_depth)
+            sampler._ring = (batch_size, batch_cap, ring_depth)
             while sampler._open_epoch is token and sampler.ring_pop(buf) > 0:
                 yield buf
         else:
@@ -118,6 +217,7 @@ def stream_epoch(sampler, data, batch_size, batch_cap, ring_depth=16):
     finally:
         if sampler._open_epoch is token:
             sampler._open_epoch = None
+            sampler._ring = None
             sampler.ring_stop()
             sampler.push_state()
 
