@@ -16,7 +16,7 @@
  *     (the reference's torch.cat([user_emb, item_emb]), LightGCN.py:69).
  *   - adjacency: CSR, int32 rowptr[n+1], int32 colidx[nnz], fp32 vals[nnz]
  *     (scipy CSR of data/graph.py:10-24, indices sorted within a row).
- *   - d (embedding.size) must be one of 32, 64, 128, 256.
+ *   - d (embedding.size) must be one of 16, 32, 64, 128, 256.
  */
 #ifndef SELFREC_B200_H
 #define SELFREC_B200_H

@@ -208,11 +208,12 @@ int scatter_segments(float* dst, int d, const ScatterSegs& segs, cudaStream_t st
   return split ? launch_kernel(scatter_add_rows_kernel<D, true>, grid, 256, 0, st, "scatter_add_rows_kernel", dst, segs)        \
                : launch_kernel(scatter_add_rows_kernel<D, false>, grid, 256, 0, st, "scatter_add_rows_kernel", dst, segs);
   switch (d) {
+    case 16: SRB_SCATTER(16)
     case 32: SRB_SCATTER(32)
     case 64: SRB_SCATTER(64)
     case 128: SRB_SCATTER(128)
     case 256: SRB_SCATTER(256)
-    default: set_error("scatter: unsupported d=%d (32, 64, 128, 256)", d); return SRB_ERR_ARG;
+    default: set_error("scatter: unsupported d=%d (16, 32, 64, 128, 256)", d); return SRB_ERR_ARG;
   }
 #undef SRB_SCATTER
 }
@@ -335,12 +336,13 @@ extern "C" int srb_bpr_l2_fwd_bwd(const srb_bpr_desc* d, void* stream) {
   case DD:                                                                                           \
     SRB_TRY(srb::launch_kernel(srb::bpr_reduce_kernel<DD>, blocks, 256, 0, st, "bpr_reduce_kernel", a)); \
     return srb::launch_kernel(srb::bpr_grad_kernel<DD>, blocks, 256, 0, st, "bpr_grad_kernel", a);
+    SRB_CASE(16)
     SRB_CASE(32)
     SRB_CASE(64)
     SRB_CASE(128)
     SRB_CASE(256)
 #undef SRB_CASE
-    default: srb::set_error("bpr: unsupported d=%d (32, 64, 128, 256)", d->d); return SRB_ERR_ARG;
+    default: srb::set_error("bpr: unsupported d=%d (16, 32, 64, 128, 256)", d->d); return SRB_ERR_ARG;
   }
 }
 

@@ -503,7 +503,7 @@ extern "C" int srb_train_step(const srb_step_desc* s, void* stream) {
   using namespace srb;
   SRB_REQUIRE(s != nullptr, "step: null desc");
   SRB_REQUIRE(s->model >= SRB_MODEL_MF && s->model <= SRB_MODEL_SGL, "step: unknown model %d", s->model);
-  SRB_REQUIRE(s->d == 32 || s->d == 64 || s->d == 128 || s->d == 256, "step: unsupported d=%d (32, 64, 128, 256)", s->d);
+  SRB_REQUIRE(s->d == 16 || s->d == 32 || s->d == 64 || s->d == 128 || s->d == 256, "step: unsupported d=%d (16, 32, 64, 128, 256)", s->d);
   SRB_REQUIRE(s->n_users > 0 && s->n_items > 0 && s->batch_cap > 0, "step: bad sizes");
   SRB_REQUIRE(s->params && s->adam_m && s->adam_v && s->step_dev && s->scalars && s->losses && s->batch, "step: null pointer");
   SRB_REQUIRE(s->model == SRB_MODEL_MF || s->n_layers >= 1, "step: graph models need n_layers >= 1");

@@ -826,7 +826,7 @@ extern "C" int srb_infonce_fwd_bwd(const srb_infonce_desc* d, void* stream) {
   SRB_REQUIRE(d != nullptr, "infonce: null desc");
   SRB_REQUIRE(d->n_problems >= 1 && d->n_problems <= 4, "infonce: n_problems must be 1..4");
   SRB_REQUIRE(d->temperature > 0.f, "infonce: temperature must be positive");
-  SRB_REQUIRE(d->d == 32 || d->d == 64 || d->d == 128 || d->d == 256, "infonce: unsupported d=%d (32, 64, 128, 256)", d->d);
+  SRB_REQUIRE(d->d == 16 || d->d == 32 || d->d == 64 || d->d == 128 || d->d == 256, "infonce: unsupported d=%d (16, 32, 64, 128, 256)", d->d);
   int max_n = 0;
   for (int q = 0; q < d->n_problems; ++q) {
     const srb_infonce_problem& s = d->prob[q];
@@ -893,6 +893,7 @@ extern "C" int srb_infonce_fwd_bwd(const srb_infonce_desc* d, void* stream) {
   // the tensor-core LSE pass shifts by the bound 1/tau of a cosine logit: needs exp(-2/tau) representable
   if (d->d == 64 && d->b_cos && d->n_problems <= 2 && a.inv_tau <= 40.f) return srb::nce_launch_tc(a, d->n_problems, st);
   switch (d->d) {
+    case 16: return srb::nce_launch<16>(a, d->n_problems, st);
     case 32: return srb::nce_launch<32>(a, d->n_problems, st);
     case 64: return srb::nce_launch<64>(a, d->n_problems, st);
     case 128: return srb::nce_launch<128>(a, d->n_problems, st);

@@ -376,11 +376,12 @@ extern "C" int srb_score_topk(const srb_topk_desc* d, void* stream) {
   a.n_q_dev = nullptr;
   a.q_skip = 0;
   switch (d->d) {
+    case 16: return srb::launch_topk<16>(a, (cudaStream_t)stream);
     case 32: return srb::launch_topk<32>(a, (cudaStream_t)stream);
     case 64: return srb::launch_topk<64>(a, (cudaStream_t)stream);
     case 128: return srb::launch_topk<128>(a, (cudaStream_t)stream);
     case 256: return srb::launch_topk<256>(a, (cudaStream_t)stream);  // 164 KB of shared memory (opt-in)
-    default: srb::set_error("topk: unsupported d=%d (32, 64, 128, 256)", d->d); return SRB_ERR_ARG;
+    default: srb::set_error("topk: unsupported d=%d (16, 32, 64, 128, 256)", d->d); return SRB_ERR_ARG;
   }
 }
 
@@ -402,11 +403,12 @@ extern "C" int srb_score_rows(const float* user_emb, const float* item_emb, int3
   dim3 grid((n_items + 255) / 256, n_q);
   cudaStream_t st = (cudaStream_t)stream;
   switch (d) {
+    case 16: srb::score_rows_kernel<16><<<grid, 256, 0, st>>>(user_emb, item_emb, users, n_items, out); break;
     case 32: srb::score_rows_kernel<32><<<grid, 256, 0, st>>>(user_emb, item_emb, users, n_items, out); break;
     case 64: srb::score_rows_kernel<64><<<grid, 256, 0, st>>>(user_emb, item_emb, users, n_items, out); break;
     case 128: srb::score_rows_kernel<128><<<grid, 256, 0, st>>>(user_emb, item_emb, users, n_items, out); break;
     case 256: srb::score_rows_kernel<256><<<grid, 256, 0, st>>>(user_emb, item_emb, users, n_items, out); break;
-    default: srb::set_error("score_rows: unsupported d=%d (32, 64, 128, 256)", d); return SRB_ERR_ARG;
+    default: srb::set_error("score_rows: unsupported d=%d (16, 32, 64, 128, 256)", d); return SRB_ERR_ARG;
   }
   return srb::post_launch("score_rows_kernel");
 }

@@ -609,11 +609,12 @@ static int gather(const Ctx& c, const float* utab, const float* itab, int64_t ct
   const int slots = (sec_hi - sec_lo) * c.B;
   const int blocks = (slots + 7) / 8;
   switch (c.d) {
+    case 16: shard_gather_kernel<16><<<blocks, 256, 0, c.st>>>(g); break;
     case 32: shard_gather_kernel<32><<<blocks, 256, 0, c.st>>>(g); break;
     case 64: shard_gather_kernel<64><<<blocks, 256, 0, c.st>>>(g); break;
     case 128: shard_gather_kernel<128><<<blocks, 256, 0, c.st>>>(g); break;
     case 256: shard_gather_kernel<256><<<blocks, 256, 0, c.st>>>(g); break;
-    default: set_error("shard gather: unsupported d=%d (32, 64, 128, 256)", c.d); return SRB_ERR_ARG;
+    default: set_error("shard gather: unsupported d=%d (16, 32, 64, 128, 256)", c.d); return SRB_ERR_ARG;
   }
   return post_launch("shard_gather_kernel");
 }
@@ -623,7 +624,7 @@ static int make_ctx(const srb_shard_desc* s, void* stream, Ctx& c) {
   SRB_REQUIRE(s->model == SRB_MODEL_LIGHTGCN || s->model == SRB_MODEL_SIMGCL || s->model == SRB_MODEL_XSIMGCL || s->model == SRB_MODEL_SGL,
               "shard: the sharded step covers LightGCN, SimGCL, XSimGCL and SGL (model %d)", s->model);
   SRB_REQUIRE(s->world >= 1 && s->world <= 8 && s->rank >= 0 && s->rank < s->world, "shard: bad world/rank %d/%d", s->world, s->rank);
-  SRB_REQUIRE(s->d == 32 || s->d == 64 || s->d == 128 || s->d == 256, "shard: unsupported d=%d (32, 64, 128, 256)", s->d);
+  SRB_REQUIRE(s->d == 16 || s->d == 32 || s->d == 64 || s->d == 128 || s->d == 256, "shard: unsupported d=%d (16, 32, 64, 128, 256)", s->d);
   SRB_REQUIRE(s->n_users > 0 && s->n_items > 0 && s->batch_cap > 0 && s->n_layers >= 1, "shard: bad sizes");
   SRB_REQUIRE(s->noise_mode == 0 || s->noise_mode == 2, "shard: noise comes from the in-kernel Philox stream (noise_mode 2)");
   SRB_REQUIRE(s->model != SRB_MODEL_SGL || s->noise_mode == 0, "shard: SGL adds no noise (noise_mode 0)");

@@ -162,8 +162,8 @@ __device__ __forceinline__ void spmm_epilogue(const SpmmArgs& a, int row, int gl
 }
 
 // Mapping: a row vector of D floats lives on LPR = D/8 lanes (two float4 per lane: columns
-// [4*gl, 4*gl+4) and [D/2 + 4*gl, ...)), so a warp holds 32/LPR lane groups: 8 at D = 32, one (the whole warp) at
-// D = 256.  Rows are taken in `row_order` (degree-descending), in three
+// [4*gl, 4*gl+4) and [D/2 + 4*gl, ...)), so a warp holds 32/LPR lane groups: 16 at D = 16, 8 at D = 32, one (the whole
+// warp) at D = 256.  Rows are taken in `row_order` (degree-descending), in three
 // classes so that no row is a long chain of dependent L2 round trips (a row of thousands of non-zeros handled by
 // one warp alone would take as long as the rest of the matrix):
 //   * the first n_vlong rows get a whole CTA: 8 warps x 32/LPR lane groups stride through the row, partial
@@ -597,11 +597,12 @@ int launch_rows_epilogue(const SpmmArgs& a, int d, cudaStream_t st) {
   if (blocks > cap) blocks = cap;
   if (blocks < 1) blocks = 1;
   switch (d) {
+    case 16: return launch_kernel(rows_epilogue_kernel<16>, (int)blocks, 256, 0, st, "rows_epilogue_kernel", a);
     case 32: return launch_kernel(rows_epilogue_kernel<32>, (int)blocks, 256, 0, st, "rows_epilogue_kernel", a);
     case 64: return launch_kernel(rows_epilogue_kernel<64>, (int)blocks, 256, 0, st, "rows_epilogue_kernel", a);
     case 128: return launch_kernel(rows_epilogue_kernel<128>, (int)blocks, 256, 0, st, "rows_epilogue_kernel", a);
     case 256: return launch_kernel(rows_epilogue_kernel<256>, (int)blocks, 256, 0, st, "rows_epilogue_kernel", a);
-    default: set_error("rows_epilogue: unsupported d=%d (32, 64, 128, 256)", d); return SRB_ERR_ARG;
+    default: set_error("rows_epilogue: unsupported d=%d (16, 32, 64, 128, 256)", d); return SRB_ERR_ARG;
   }
 }
 
@@ -613,11 +614,12 @@ int launch_reduce_rows(const SpmmArgs& a, const ReduceArgs& r, int d, cudaStream
   if (blocks > cap) blocks = cap;
   if (blocks < 1) blocks = 1;
   switch (d) {
+    case 16: reduce_rows_kernel<16><<<(int)blocks, 256, 0, st>>>(a, r); break;
     case 32: reduce_rows_kernel<32><<<(int)blocks, 256, 0, st>>>(a, r); break;
     case 64: reduce_rows_kernel<64><<<(int)blocks, 256, 0, st>>>(a, r); break;
     case 128: reduce_rows_kernel<128><<<(int)blocks, 256, 0, st>>>(a, r); break;
     case 256: reduce_rows_kernel<256><<<(int)blocks, 256, 0, st>>>(a, r); break;
-    default: set_error("reduce_rows: unsupported d=%d (32, 64, 128, 256)", d); return SRB_ERR_ARG;
+    default: set_error("reduce_rows: unsupported d=%d (16, 32, 64, 128, 256)", d); return SRB_ERR_ARG;
   }
   return post_launch("reduce_rows_kernel");
 }
@@ -656,11 +658,12 @@ int launch_spmm(const SpmmArgs& a, int d, cudaStream_t st) {
   long long hub_blocks = a.seg ? (a.n_cta > 0 ? a.n_cta : (a.n_work > 0 ? 1 : 0)) : a.n_work;  // (device-counted lists: the capacity)
   if (hub_blocks > cap) hub_blocks = cap;
   switch (d) {
+    case 16: return launch_spmm_d<16>(a, (int)hub_blocks, (int)blocks, st);
     case 32: return launch_spmm_d<32>(a, (int)hub_blocks, (int)blocks, st);
     case 64: return launch_spmm_d<64>(a, (int)hub_blocks, (int)blocks, st);
     case 128: return launch_spmm_d<128>(a, (int)hub_blocks, (int)blocks, st);
     case 256: return launch_spmm_d<256>(a, (int)hub_blocks, (int)blocks, st);
-    default: set_error("spmm: unsupported d=%d (32, 64, 128, 256)", d); return SRB_ERR_ARG;
+    default: set_error("spmm: unsupported d=%d (16, 32, 64, 128, 256)", d); return SRB_ERR_ARG;
   }
 }
 

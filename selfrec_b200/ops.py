@@ -12,7 +12,7 @@ import torch
 from . import _lib
 from ._lib import SrbError
 
-_SUPPORTED_D = (32, 64, 128, 256)
+_SUPPORTED_D = (16, 32, 64, 128, 256)
 LONG_ROW_NNZ = 64    # rows at least this long are processed by a whole warp (srb_spmm_desc.n_long_rows)
 VLONG_ROW_NNZ = 256  # rows at least this long are processed by a whole CTA (srb_spmm_desc.n_vlong_rows)
 
@@ -278,7 +278,7 @@ def _spmm_raw(adj, x, y=None, _entry="srb_spmm_csr", **epi):
     if x.shape[0] != n_cols:
         raise ValueError(f"spmm: A is {adj.shape} but X has {x.shape[0]} rows")
     if d not in _SUPPORTED_D:
-        raise SrbError(f"spmm: embedding size {d} unsupported (32, 64, 128, 256)")
+        raise SrbError(f"spmm: embedding size {d} unsupported (16, 32, 64, 128, 256)")
     desc = _lib.SpmmDesc()
     desc.rowptr, desc.colidx, desc.vals = _p(adj.rowptr), _p(adj.colidx), _p(adj.vals)
     desc.row_order = _p(adj.row_order)
@@ -478,7 +478,7 @@ class _InfoNceFn(torch.autograd.Function):
             raise ValueError("InfoNCE: views must have the same shape")
         n, d = v1.shape
         if d not in _SUPPORTED_D:
-            raise SrbError(f"InfoNCE: embedding size {d} unsupported (32, 64, 128, 256)")
+            raise SrbError(f"InfoNCE: embedding size {d} unsupported (16, 32, 64, 128, 256)")
         idx = torch.arange(n, device=v1.device, dtype=torch.int32)
         losses, outs = infonce_raw([dict(table1=v1, table2=v2, idx=idx, n=n, weight=1.0)], d, temperature, b_cos)
         ctx.save_for_backward(*outs[0])

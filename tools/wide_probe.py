@@ -1,5 +1,6 @@
 """Embedding width on the yelp2018 shape: XSimGCL and LightGCN steps/s, workspace size and full-catalogue rank time at
-d = 64, 128, 256, with the card's name and power limit read in the same run.  One JSON line on stdout.
+the widths of --dims (any of 16, 32, 64, 128, 256), with the card's name and power limit read in the same run.  One
+JSON line on stdout.
 
     python tools/wide_probe.py [--dims 64,128,256] [--window 1.0]
 
