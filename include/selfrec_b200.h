@@ -630,6 +630,47 @@ int srb_shard_step(const srb_shard_desc* desc, void* stream);
  * lands in every rank's symmetric region at item_final */
 int srb_shard_forward(const srb_shard_desc* desc, float* out_user, void* stream);
 
+/* ---- neighbourhood baselines: ItemKNN / UserKNN (model/graph/ItemKNN.py, model/graph/UserKNN.py) ---------------- */
+#define SRB_KNN_MAX_TOPK 1024
+
+/* Rows of a binary CSR A (ItemKNN: items -> users; UserKNN: users -> items) compared with each other through the
+ * transpose T.  rank[r]: position of row r's name in Python's sorted() of the row names, the second key of
+ * heapq.nlargest over (sim, name) tuples (ItemKNN.py:51, UserKNN.py:53).  Device pointers, int32. */
+typedef struct srb_knn_rows {
+  const int32_t* row_ptr; /* [n_rows + 1] */
+  const int32_t* row_idx;
+  const int32_t* t_ptr;   /* [n_cols + 1] */
+  const int32_t* t_idx;
+  const int32_t* rank;    /* [n_rows] */
+  int32_t n_rows;
+} srb_knn_rows;
+
+int64_t srb_knn_neighbors_workspace_bytes(int32_t n_rows);
+/* ItemKNN.py:14-56 / UserKNN.py:14-57, train(): for every row a, c(a, b) = |A[a] ∩ A[b]| over b != a, and
+ *   sim = (c / (c + shrinkage)) * (c / (sqrt(|A[a]|) * sqrt(|A[b]|) + 1e-8)),
+ * each operation one correctly rounded float64 step in that order.  Candidates are the b with c >= 1; the row keeps
+ * the topk best by (sim desc, rank desc).  out_id / out_sim: [n_rows, topk], entries past out_cnt[a] are -1 / 0.
+ * topk in 1..SRB_KNN_MAX_TOPK, shrinkage in 0..2^52; workspace: srb_knn_neighbors_workspace_bytes (a count and a
+ * candidate list of n_rows int32 per CTA, no n_rows^2 buffer). */
+int srb_knn_neighbors(const srb_knn_rows* rows, int32_t topk, int64_t shrinkage, int32_t* out_id, double* out_sim,
+                      int32_t* out_cnt, void* workspace, int64_t workspace_bytes, void* stream);
+/* ItemKNN.py:58-81 (mode 0) / UserKNN.py:59-80 (mode 1), predict(u) for the listed user ids: out[q] = float64
+ * [n_items] row.  Mode 0: seq = each user's items in training_set_u order, the neighbour table is the items'; the
+ * sims of item i's neighbours are added for every i in seq[u], in that order.  Mode 1: seq = each user's items, the
+ * table is the users'; for each neighbour v of u in list order its sim is added to every item of seq[v].  Then
+ * out = acc / (acc + 1e-8).  With rated_ptr / rated_idx (both or neither) rated items become -10e8
+ * (base/graph_recommender.py:49-50). */
+int srb_knn_score_rows(int32_t mode, const int32_t* users, int32_t n_q, int32_t n_items, const int32_t* nbr_id,
+                       const double* nbr_sim, const int32_t* nbr_cnt, int32_t topk, const int32_t* seq_ptr,
+                       const int32_t* seq_idx, const int32_t* rated_ptr, const int32_t* rated_idx, double* out,
+                       void* stream);
+int64_t srb_topk_f64_workspace_bytes(int32_t n_q, int32_t k);
+/* find_k_largest(k, row) of util/algorithm.py:144-156 on float64 rows [n_q, n_items], k in 1..n_items: heapify of the
+ * first k (score, id) tuples, heapreplace iff score > heap[0] score, then numba's quicksort argsort by score,
+ * descending.  Ties come out in the reference's order, which depends on the heap's array layout. */
+int srb_topk_rows_f64(const double* rows, int32_t n_q, int32_t n_items, int32_t k, int32_t* out_ids, double* out_scores,
+                      void* workspace, int64_t workspace_bytes, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -27,14 +27,14 @@ _DROPIN = {
     "data.loader": "selfrec_b200.data.loader",
     "util.evaluation": "selfrec_b200.util.evaluation",
 }
-_FUSED_MODELS = {f"model.graph.{m}": f"selfrec_b200.model.graph.{m}" for m in ("MF", "LightGCN", "SimGCL", "XSimGCL", "SGL")}
+_FUSED_MODELS = {f"model.graph.{m}": f"selfrec_b200.model.graph.{m}" for m in ("MF", "LightGCN", "SimGCL", "XSimGCL", "SGL", "ItemKNN", "UserKNN")}
 
 
 def install(fused_models=True):
     """Register the drop-in modules under the reference's import names.
 
     With fused_models=True the five in-scope model classes resolve to the fused-engine
-    versions too; with False the reference's own model files run on top of the five
+    versions too, and ItemKNN / UserKNN to their GPU versions; with False the reference's own model files run on top of the five
     boundary modules (op-level drop-in)."""
     if "WORLD_SIZE" in os.environ:  # started by torchrun: one process per GPU
         _init_process_group()

@@ -138,6 +138,12 @@ class ShardLayout(C.Structure):
                 ("ctrl", C.c_int64)]
 
 
+class KnnRows(C.Structure):
+    _fields_ = [("row_ptr", VP), ("row_idx", VP), ("t_ptr", VP), ("t_idx", VP), ("rank", VP), ("n_rows", C.c_int32)]
+
+
+KNN_MAX_TOPK = 1024  # SRB_KNN_MAX_TOPK
+
 MODEL_IDS = {"MF": 0, "LightGCN": 1, "SimGCL": 2, "XSimGCL": 3, "SGL": 4}
 BATCH_HEADER = 4
 
@@ -198,6 +204,11 @@ SYMBOLS = {
                                  C.POINTER(ShardLayout)]),
     "srb_shard_step": (C.c_int, [C.POINTER(ShardDesc), VP]),
     "srb_shard_forward": (C.c_int, [C.POINTER(ShardDesc), VP, VP]),
+    "srb_knn_neighbors_workspace_bytes": (C.c_int64, [C.c_int32]),
+    "srb_knn_neighbors": (C.c_int, [C.POINTER(KnnRows), C.c_int32, C.c_int64, VP, VP, VP, VP, C.c_int64, VP]),
+    "srb_knn_score_rows": (C.c_int, [C.c_int32, VP, C.c_int32, C.c_int32, VP, VP, VP, C.c_int32, VP, VP, VP, VP, VP, VP]),
+    "srb_topk_f64_workspace_bytes": (C.c_int64, [C.c_int32, C.c_int32]),
+    "srb_topk_rows_f64": (C.c_int, [VP, C.c_int32, C.c_int32, C.c_int32, VP, VP, VP, C.c_int64, VP]),
 }
 
 _lib = None

@@ -20,7 +20,7 @@ LIB = os.path.join(HERE, "libselfrec_b200.so")
 STAMP = os.path.join(HERE, "libselfrec_b200.stamp")  # no leading dot: it has to travel with the .so
 LOCK = os.path.join(HERE, "libselfrec_b200.lock")
 
-SOURCES = ["capi.cu", "spmm.cu", "bpr.cu", "infonce.cu", "score_topk.cu", "score_topk_tc.cu", "engine.cu", "sharded.cu", "graphbuild.cu", "sampler.cpp", "dataset.cpp"]
+SOURCES = ["capi.cu", "spmm.cu", "bpr.cu", "infonce.cu", "score_topk.cu", "score_topk_tc.cu", "engine.cu", "sharded.cu", "graphbuild.cu", "knn.cu", "sampler.cpp", "dataset.cpp"]
 ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]
 NVCC_FLAGS = ARCH + [
     "-O3", "-std=c++17", "-lineinfo",

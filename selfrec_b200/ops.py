@@ -599,6 +599,95 @@ def topk_rows(scores, k):
 
 
 # ----------------------------------------------------------------------------------------
+# neighbourhood baselines (ItemKNN / UserKNN)
+# ----------------------------------------------------------------------------------------
+def _i32c(t, name):
+    if not isinstance(t, torch.Tensor):
+        raise TypeError(f"{name}: expected a torch.Tensor")
+    if not t.is_cuda:
+        raise SrbError(f"{name}: selfrec_b200 ops need CUDA tensors (no CPU fallback)")
+    if t.dtype != torch.int32:
+        raise TypeError(f"{name}: expected int32, got {t.dtype}")
+    t = t.contiguous()
+    return t if t.numel() else torch.zeros(1, dtype=torch.int32, device=t.device)  # an empty list still needs an address
+
+
+def knn_neighbors(row_ptr, row_idx, t_ptr, t_idx, rank, topk, shrinkage):
+    """Neighbour table of the rows of a binary CSR (row_ptr, row_idx) against each other through its transpose (t_ptr,
+    t_idx): the topk rows b != a of largest (sim, rank[b]), sim as in ItemKNN.py:14-30.  Device int32 inputs.
+    Returns (ids int32 [n_rows, topk], sims float64 [n_rows, topk], counts int32 [n_rows]); entries past counts[a]
+    are -1 / 0."""
+    lib = _lib.require_device()
+    topk, shrinkage = int(topk), int(shrinkage)
+    if not 1 <= topk <= _lib.KNN_MAX_TOPK:
+        raise SrbError(f"knn_neighbors: topK={topk} outside 1..{_lib.KNN_MAX_TOPK}")
+    if shrinkage < 0:
+        raise SrbError(f"knn_neighbors: shrinkage={shrinkage} must be >= 0")
+    row_ptr, row_idx = _i32c(row_ptr, "knn row_ptr"), _i32c(row_idx, "knn row_idx")
+    t_ptr, t_idx, rank = _i32c(t_ptr, "knn t_ptr"), _i32c(t_idx, "knn t_idx"), _i32c(rank, "knn rank")
+    n = row_ptr.numel() - 1
+    if n < 1 or rank.numel() != n:
+        raise SrbError(f"knn_neighbors: {n} rows and {rank.numel()} name ranks")
+    dev = row_ptr.device
+    rows = _lib.KnnRows(_p(row_ptr), _p(row_idx), _p(t_ptr), _p(t_idx), _p(rank), n)
+    ws_bytes = int(lib.srb_knn_neighbors_workspace_bytes(n))
+    ws = torch.empty(ws_bytes, dtype=torch.uint8, device=dev)
+    ids = torch.empty((n, topk), dtype=torch.int32, device=dev)
+    sims = torch.empty((n, topk), dtype=torch.float64, device=dev)
+    cnt = torch.empty(n, dtype=torch.int32, device=dev)
+    _lib.check(lib.srb_knn_neighbors(C.byref(rows), topk, shrinkage, _p(ids), _p(sims), _p(cnt), _p(ws), ws_bytes, _stream()),
+               "srb_knn_neighbors")
+    return ids, sims, cnt
+
+
+KNN_ITEM, KNN_USER = 0, 1  # srb_knn_score_rows modes
+
+
+def knn_score_rows(mode, users, n_items, table, seq_ptr, seq_idx, rated_ptr=None, rated_idx=None):
+    """Float64 predict() rows [len(users), n_items] of ItemKNN (mode KNN_ITEM: seq = each user's items in training_set_u
+    order, table = the items' neighbours) or UserKNN (KNN_USER: seq = each user's items, table = the users' neighbours);
+    table = knn_neighbors(...).  With rated_ptr / rated_idx the rated items are set to -10e8."""
+    lib = _lib.require_device()
+    ids, sims, cnt = table
+    if mode not in (KNN_ITEM, KNN_USER):
+        raise SrbError(f"knn_score_rows: mode={mode} (KNN_ITEM or KNN_USER)")
+    if sims.dtype != torch.float64 or not sims.is_cuda or sims.shape != ids.shape:
+        raise SrbError("knn_score_rows: the table's sims must be a CUDA float64 tensor shaped like its ids")
+    dev = ids.device
+    users = _i32(users, dev)
+    n_q = users.numel()
+    users = _i32c(users, "knn users")
+    if (rated_ptr is None) != (rated_idx is None):
+        raise SrbError("knn_score_rows: rated_ptr and rated_idx go together")
+    rp = None if rated_ptr is None else _i32c(_i32(rated_ptr, dev), "knn rated_ptr")
+    ri = None if rated_idx is None else _i32c(_i32(rated_idx, dev), "knn rated_idx")
+    seq_ptr, seq_idx = _i32c(_i32(seq_ptr, dev), "knn seq_ptr"), _i32c(_i32(seq_idx, dev), "knn seq_idx")
+    out = torch.empty((n_q, int(n_items)), dtype=torch.float64, device=dev)
+    _lib.check(lib.srb_knn_score_rows(mode, _p(users), n_q, int(n_items), _p(ids.contiguous()), _p(sims.contiguous()), _p(_i32c(cnt, "knn counts")),
+                                      ids.shape[1], _p(seq_ptr), _p(seq_idx), _p(rp), _p(ri), _p(out), _stream()), "srb_knn_score_rows")
+    return out
+
+
+def topk_rows_f64(rows, k):
+    """find_k_largest(k, row) of util/algorithm.py:144-156 for every float64 row of rows [n_q, n_items], ties in the
+    reference's heap-and-quicksort order; k in 1..n_items.  Returns (ids int32 [n_q, k], scores float64 [n_q, k])."""
+    lib = _lib.require_device()
+    if not isinstance(rows, torch.Tensor) or not rows.is_cuda or rows.dtype != torch.float64 or rows.dim() != 2:
+        raise SrbError("topk_rows_f64: expected a CUDA float64 [n_q, n_items] tensor")
+    rows = rows.contiguous()
+    n_q, n_items = rows.shape
+    k = int(k)
+    if not 1 <= k <= n_items:
+        raise SrbError(f"topk_rows_f64: k={k} outside 1..n_items={n_items}")
+    ws_bytes = int(lib.srb_topk_f64_workspace_bytes(n_q, k))
+    ws = torch.empty(max(ws_bytes, 1), dtype=torch.uint8, device=rows.device)
+    out_ids = torch.empty((n_q, k), dtype=torch.int32, device=rows.device)
+    out_sc = torch.empty((n_q, k), dtype=torch.float64, device=rows.device)
+    _lib.check(lib.srb_topk_rows_f64(_p(rows), n_q, n_items, k, _p(out_ids), _p(out_sc), _p(ws), ws_bytes, _stream()), "srb_topk_rows_f64")
+    return out_ids, out_sc
+
+
+# ----------------------------------------------------------------------------------------
 # Adam
 # ----------------------------------------------------------------------------------------
 def adam_prepare(step_dev, scalars, lr, beta1=0.9, beta2=0.999):
