@@ -328,14 +328,16 @@ typedef struct srb_topk_desc {
   int32_t k;
   int32_t* out_ids;
   float* out_scores;
-  int32_t impl; /* 0 auto; 1 CUDA cores, exact fp32; 2 wgmma TF32 candidate lists (2 x 24 per user) + exact fp32
+  int32_t impl; /* 0 auto (impl 2 when d is 64 or 128, n_items >= 1024 and a workspace is given, else impl 1);
+                   1 CUDA cores, exact fp32; 2 (d = 64 or 128) wgmma TF32 candidate lists (2 x 24 per user) + exact fp32
                    rescoring + a per-user exactness certificate, uncertified users re-run by the exact path */
-  void* workspace; /* impl 2: srb_topk_workspace_bytes */
+  void* workspace; /* impl 2: srb_topk_workspace_bytes(n_q, n_items, d, k) bytes, 256-byte aligned */
   int64_t workspace_bytes;
 } srb_topk_desc;
 
 int64_t srb_topk_workspace_bytes(int32_t n_q, int32_t n_items, int32_t d, int32_t k);
-/* byte offset (inside the impl-2 workspace) of the int32 count of users the exact fallback re-ran */
+/* byte offset (inside the impl-2 workspace) of the int32 count of users the exact fallback re-ran; the same at
+   d = 64 and d = 128 */
 int64_t srb_topk_fallback_count_offset(int32_t n_q, int32_t n_items);
 int srb_score_topk(const srb_topk_desc* desc, void* stream);
 /* Dense score rows out[q, i] = <user_emb[users[q]], item_emb[i]>, the reference's predict()

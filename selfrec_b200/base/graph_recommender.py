@@ -70,9 +70,15 @@ class GraphRecommender(Recommender):
         if self._has_embedding_tables():
             ids, scores = ops.score_topk(self.user_emb.detach(), self.item_emb.detach(), uids, rated_ptr, rated_idx, self.max_N)
             return names, ids.cpu().numpy(), scores.cpu().numpy()
-        # generic models: their own predict(), batched through the CUDA row top-k
-        ids_out = np.empty((len(names), self.max_N), dtype=np.int32)
-        sc_out = np.empty((len(names), self.max_N), dtype=np.float32)
+        ids, sc = self._predict_topk(names, uids, self.max_N)
+        return names, ids.cpu().numpy(), sc.cpu().numpy()
+
+    def _predict_topk(self, names, uids, n):
+        """Generic models: their own predict() rows, rated items masked, batched through the CUDA row top-k.
+        (ids int32 [len(names), n], scores fp32) on the device."""
+        rated_ptr, rated_idx = self.data.rated_csr()
+        ids_out = torch.empty((len(names), n), dtype=torch.int32, device="cuda")
+        sc_out = torch.empty((len(names), n), dtype=torch.float32, device="cuda")
         step = 512
         for s in range(0, len(names), step):
             rows = np.stack([np.asarray(self.predict(u), dtype=np.float32) for u in names[s:s + step]])
@@ -80,13 +86,18 @@ class GraphRecommender(Recommender):
                 rows[r, rated_idx[rated_ptr[uid]:rated_ptr[uid + 1]]] = -10e8
             dev_rows = torch.from_numpy(rows).cuda()
             parts = []
-            for lo in range(0, self.max_N, ops.TOPK_KERNEL_MAX):  # 32 per pass, winners struck out (ops._score_topk_wide)
-                ids, sc = ops.topk_rows(dev_rows, min(ops.TOPK_KERNEL_MAX, self.max_N - lo))
+            for lo in range(0, n, ops.TOPK_KERNEL_MAX):  # 32 per pass, winners struck out (ops._score_topk_wide)
+                ids, sc = ops.topk_rows(dev_rows, min(ops.TOPK_KERNEL_MAX, n - lo))
                 parts.append((ids, sc))
                 dev_rows.scatter_(1, ids.long(), float("-inf"))
-            ids, sc = torch.cat([p[0] for p in parts], 1), torch.cat([p[1] for p in parts], 1)
-            ids_out[s:s + step], sc_out[s:s + step] = ids.cpu().numpy(), sc.cpu().numpy()
-        return names, ids_out, sc_out
+            ids_out[s:s + step], sc_out[s:s + step] = torch.cat([p[0] for p in parts], 1), torch.cat([p[1] for p in parts], 1)
+        return ids_out, sc_out
+
+    def export_recommendations(self, out_dir, top_n=None, users=None, chunk=None):
+        """Write the top-N lists (default N = max_N) of `users` (names; default every training user) under out_dir,
+        rated items masked as in test(); returns the export directory (export.py describes the format)."""
+        from .. import export
+        return export.export_recommendations(self, out_dir, top_n=top_n, users=users, chunk=chunk)
 
     def test(self):
         names, ids, scores = self.rank_all()
@@ -115,6 +126,12 @@ class GraphRecommender(Recommender):
         if main:
             FileIO.write_file(out_dir, f"{name}@{stamp}-performance.txt", self.result)
             print(f"The result of {self.model_name}:\n{''.join(self.result)}")
+        conf = self.config
+        if conf.contain("export.dir"):  # optional: every training user's top-N lists (export.topN, default max_N)
+            top_n = int(conf["export.topN"]) if conf.contain("export.topN") else None
+            path = self.export_recommendations(conf["export.dir"], top_n=top_n)
+            if main:
+                print("The recommendation lists have been exported to ", abspath(path), ".")
 
     def _fast_measure(self):
         """fast_evaluation's metrics without leaving id space: full-catalog top-k on the device, hit masks on

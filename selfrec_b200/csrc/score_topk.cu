@@ -319,11 +319,12 @@ __global__ void __launch_bounds__(256) fb_topk_kernel(const float* scratch, cons
   }
 }
 
-int score_topk_fallback(const srb_topk_desc* d, const int32_t* fb_users, const int32_t* fb_rows, const int32_t* fb_count,
-                        float* scratch, int fb_cap, cudaStream_t st) {
+template <int D>
+static int score_topk_fallback_d(const srb_topk_desc* d, const int32_t* fb_users, const int32_t* fb_rows, const int32_t* fb_count,
+                                 float* scratch, int fb_cap, cudaStream_t st) {
   // fast path: up to fb_cap users
   dim3 grid((d->n_items + 255) / 256, fb_cap < 8 ? fb_cap : 8);
-  fb_score_kernel<64><<<grid, 256, 0, st>>>(d->user_emb, d->item_emb, fb_users, fb_count, d->rated_ptr, d->rated_idx, d->n_items,
+  fb_score_kernel<D><<<grid, 256, 0, st>>>(d->user_emb, d->item_emb, fb_users, fb_count, d->rated_ptr, d->rated_idx, d->n_items,
                                             scratch, fb_cap);
   SRB_TRY(post_launch("fb_score_kernel"));
   fb_topk_kernel<<<(fb_cap + 7) / 8, 256, 0, st>>>(scratch, fb_rows, fb_count, fb_cap, d->n_items, d->k, d->out_ids, d->out_scores);
@@ -344,7 +345,13 @@ int score_topk_fallback(const srb_topk_desc* d, const int32_t* fb_users, const i
   a.q_map = fb_rows;
   a.n_q_dev = fb_count;
   a.q_skip = fb_cap;
-  return launch_topk<64>(a, st);
+  return launch_topk<D>(a, st);
+}
+
+int score_topk_fallback(const srb_topk_desc* d, const int32_t* fb_users, const int32_t* fb_rows, const int32_t* fb_count,
+                        float* scratch, int fb_cap, cudaStream_t st) {
+  if (d->d == 128) return score_topk_fallback_d<128>(d, fb_users, fb_rows, fb_count, scratch, fb_cap, st);
+  return score_topk_fallback_d<64>(d, fb_users, fb_rows, fb_count, scratch, fb_cap, st);
 }
 
 }  // namespace srb
@@ -359,7 +366,7 @@ extern "C" int srb_score_topk(const srb_topk_desc* d, void* stream) {
   SRB_REQUIRE(d->n_items >= 1 && d->n_q >= 0, "topk: bad shape");
   SRB_REQUIRE(d->impl >= 0 && d->impl <= 2, "topk: bad impl");
   if (d->n_q == 0) return SRB_OK;
-  if (d->impl == 2 || (d->impl == 0 && d->d == 64 && d->workspace != nullptr && d->n_items >= 1024))
+  if (d->impl == 2 || (d->impl == 0 && (d->d == 64 || d->d == 128) && d->workspace != nullptr && d->n_items >= 1024))
     return srb::score_topk_tc(d, (cudaStream_t)stream);
   srb::TopkArgs a;
   a.user_emb = d->user_emb;

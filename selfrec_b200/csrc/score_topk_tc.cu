@@ -4,12 +4,16 @@
 // Replaces GraphRecommender.test() base/graph_recommender.py:38-58 (predict XSimGCL.py:57-60,
 // mask :48-50, find_k_largest util/algorithm.py:144-156), same contract as impl 1.
 //
+// Both kernels are templated on the embedding size D in {64, 128}.
+//
 // Stage 1  tc_gather_kernel     users[q] rows -> contiguous [n_q, d] table (TMA cannot gather),
 //                               ||u_q||, max_i ||item_i||
 // Stage 2  tc_score_kernel      one CTA per block of UB <= 128 users, streaming the whole catalogue in
 //                               tiles of 128 items:
-//            warp 8     TMA producer: item tiles [128 x 64] fp32, 128B-swizzled, 2-stage mbarrier ring
-//            warpgroups 0, 1  (64 users each): wgmma m64n128k8 kind tf32, 8 k-steps per tile, accumulators in
+//            warp 8     TMA producer: item tiles [128 x D] fp32 in 32-float k-chunks, 128B-swizzled, through a
+//                       2-stage mbarrier ring (D = 64: a stage is a whole tile; D = 128: a stage is one k-chunk,
+//                       four stages per tile, so the 64 KB user tile fits beside the ring -- DESIGN 4.4)
+//            warpgroups 0, 1  (64 users each): wgmma m64n128k8 kind tf32, D/8 k-steps per tile, accumulators in
 //                       registers -> staged to shared memory row-major -> select: thread = one user row x one
 //                       64-column half of the tile, rated-item cursor, per-thread top-24 candidate list
 //                       (3 buckets of 8, minima in registers) in shared memory -> 2 x 24 candidates per user
@@ -19,7 +23,7 @@
 //                               (bit-identical to impl 1 / the oracle), find_k_largest's sequential
 //                               insertion in id order, and a safety test: every non-candidate of a column
 //                               half has approx score <= that half's 24th best, so the result is exact iff
-//                               thr32 := max of the two + E < exact k-th score.  Users failing it (or with fewer than
+//                               thr32 := max of the two + E(D) < exact k-th score.  Users failing it (or with fewer than
 //                               k unrated items) are re-run by the exact CUDA-core kernel (impl 1).
 #include "common.cuh"
 #include "tc_common.cuh"
@@ -28,7 +32,6 @@ namespace srb {
 
 using namespace tc;
 
-constexpr int TC_D = 64;          // embedding size handled by this kernel
 constexpr int TC_TN = 128;        // items per tile (wgmma N)
 constexpr int TC_UB = 128;        // users per CTA: two consumer warpgroups of 64 (wgmma M)
 constexpr int TC_STAGES = 2;      // smem ring depth (a tile's select takes microseconds: one tile of prefetch is enough)
@@ -36,19 +39,34 @@ constexpr int TC_LIST = 24;       // candidates per list; every user has two lis
 constexpr int TC_CAND = 2 * TC_LIST;
 constexpr int TC_THREADS = 256 + 32;   // warpgroups 0-1 MMA + select, warp 8 TMA
 constexpr int TC_SROW = TC_TN + 4;     // staged accumulator row stride (floats): conflict-free float4 row reads
-constexpr uint32_t TC_TILE_BYTES = TC_TN * TC_D * 4;     // 32 KB: 2 k-chunks x [128][32] fp32
-constexpr uint32_t TC_USER_BYTES = TC_UB * TC_D * 4;     // 32 KB: 2 k-chunks x [128][32]
+constexpr uint32_t TC_CHUNK_BYTES = 128 * 32 * 4;     // 16 KB: one k-chunk [128 rows][32] fp32 of a user or item tile
 
+// per-width layout: a tile row is D/32 k-chunks; a ring stage holds SC of them
+template <int D>
+struct TcShape {
+  static_assert(D == 64 || D == 128, "tensor-core ranking: D in {64, 128}");
+  static constexpr int KC = D / 32;                      // k-chunks per tile row
+  static constexpr int SC = (D == 64) ? 2 : 1;           // k-chunks per ring stage
+  static constexpr int SPT = KC / SC;                    // ring stages per item tile
+  static constexpr uint32_t STAGE_BYTES = SC * TC_CHUNK_BYTES;  // 32 KB (D = 64) / 16 KB (D = 128)
+  static constexpr uint32_t USER_BYTES = KC * TC_CHUNK_BYTES;   // 32 KB / 64 KB
+  // |approx - exact| <= E * ||u|| * max||i||: the TF32 operand term 2^-9 (independent of D), the accumulation term
+  // 2^-16 per 8 k-steps (it grows with the chain of k-steps: 2^-16 at D = 64, 2^-15 at D = 128) and 2^-18 for the
+  // slot tags and the final roundings (DESIGN 4.4)
+  static constexpr float E = 1.0f / 512.0f + (float)(D / 64) * (1.0f / 65536.0f) + 1.0f / 262144.0f;
+};
+
+template <int D>
 struct TcSmem {
   // dynamic shared memory, 1024-byte aligned base:
-  //   [0, 32K)          user tile    chunk c at c * 16 KB (warpgroup w's 64 rows at + w * 8 KB)
-  //   [32K, 32K+64K)    item stages  stage s, chunk c at 32K + s*32K + c*16K
+  //   [0, U)            user tile    chunk c at c * 16 KB (warpgroup w's 64 rows at + w * 8 KB); U = 32 KB / 64 KB
+  //   [U, U + 2 S)      item stages  stage s, chunk c at U + s*S + c*16K; S = 32 KB (D = 64) / 16 KB (D = 128)
   //   then the staged accumulators [2 warpgroups][64][TC_SROW] f32                  (66 KB)
   //   then candidate lists: scores [24][256] f32, ids [24][256] i32               (48 KB)
-  //   then barriers
+  //   then barriers                                          total 210 KB + 256 B at both widths
   static constexpr uint32_t users_off = 0;
-  static constexpr uint32_t items_off = TC_USER_BYTES;
-  static constexpr uint32_t stage_off = items_off + TC_STAGES * TC_TILE_BYTES;
+  static constexpr uint32_t items_off = TcShape<D>::USER_BYTES;
+  static constexpr uint32_t stage_off = items_off + TC_STAGES * TcShape<D>::STAGE_BYTES;
   static constexpr uint32_t cand_s_off = stage_off + TC_UB * TC_SROW * 4;
   static constexpr uint32_t cand_i_off = cand_s_off + TC_LIST * 2 * TC_UB * 4;
   static constexpr uint32_t bar_off = cand_i_off + TC_LIST * 2 * TC_UB * 4;
@@ -68,33 +86,54 @@ struct TcArgs {
   float* cand_thr;           // [n_q][2] min approx score of a full list, else -inf
 };
 
+template <int D>
+struct TcVec;  // the D/32 floats of a row that one lane gathers
+template <>
+struct TcVec<64> {
+  using T = float2;
+  static __device__ __forceinline__ T zero() { return make_float2(0.f, 0.f); }
+  static __device__ __forceinline__ float ss(T v) { return v.x * v.x + v.y * v.y; }
+};
+template <>
+struct TcVec<128> {
+  using T = float4;
+  static __device__ __forceinline__ T zero() { return make_float4(0.f, 0.f, 0.f, 0.f); }
+  static __device__ __forceinline__ float ss(T v) { return v.x * v.x + v.y * v.y + v.z * v.z + v.w * v.w; }
+};
+
+template <int D>
 __global__ void __launch_bounds__(256) tc_gather_kernel(const float* __restrict__ user_emb, const int32_t* __restrict__ users, int n_q,
                                                        int n_q_pad, float* __restrict__ ug, float* __restrict__ unorm,
                                                        const float* __restrict__ item_emb, int n_items, unsigned int* bmax_bits) {
   const int lane = threadIdx.x & 31;
   const int w = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
   // rows [0, n_q_pad): gathered user rows; rows [n_q_pad, n_q_pad + n_items): item norms
+  using V = TcVec<D>;
+  constexpr int PL = D / 32;  // floats per lane
   if (w < n_q_pad) {
-    float2 v = make_float2(0.f, 0.f);
-    if (w < n_q) v = *reinterpret_cast<const float2*>(user_emb + (size_t)users[w] * TC_D + lane * 2);
-    *reinterpret_cast<float2*>(ug + (size_t)w * TC_D + lane * 2) = v;
-    const float ss = warp_sum(v.x * v.x + v.y * v.y);
+    typename V::T v = V::zero();
+    if (w < n_q) v = *reinterpret_cast<const typename V::T*>(user_emb + (size_t)users[w] * D + lane * PL);
+    *reinterpret_cast<typename V::T*>(ug + (size_t)w * D + lane * PL) = v;
+    const float ss = warp_sum(V::ss(v));
     if (lane == 0 && w < n_q) unorm[w] = sqrtf(ss);
   } else if (w < n_q_pad + n_items) {
     const int i = w - n_q_pad;
-    const float2 v = *reinterpret_cast<const float2*>(item_emb + (size_t)i * TC_D + lane * 2);
-    const float ss = warp_sum(v.x * v.x + v.y * v.y);
+    const typename V::T v = *reinterpret_cast<const typename V::T*>(item_emb + (size_t)i * D + lane * PL);
+    const float ss = warp_sum(V::ss(v));
     // non-negative floats order like uints; 38 k atomics on one word serialise, so look before touching it
     const unsigned int bits = __float_as_uint(sqrtf(ss));
     if (lane == 0 && bits > *reinterpret_cast<volatile unsigned int*>(bmax_bits)) atomicMax(bmax_bits, bits);
   }
 }
 
+template <int D>
 __global__ void __launch_bounds__(TC_THREADS, 1)
 tc_score_kernel(const __grid_constant__ CUtensorMap tm_users, const __grid_constant__ CUtensorMap tm_items, const TcArgs a) {
   extern __shared__ __align__(1024) uint8_t tc_smem_raw[];
   uint8_t* sm = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(tc_smem_raw) + 1023) & ~(uintptr_t)1023);
-  uint64_t* bars = reinterpret_cast<uint64_t*>(sm + TcSmem::bar_off);
+  using Sh = TcShape<D>;
+  using Sm = TcSmem<D>;
+  uint64_t* bars = reinterpret_cast<uint64_t*>(sm + Sm::bar_off);
   uint64_t* bar_full = bars;                    // [STAGES]  TMA -> MMA
   uint64_t* bar_empty = bars + TC_STAGES;       // [STAGES]  both warpgroups' MMAs done -> TMA
   uint64_t* bar_users = bars + 2 * TC_STAGES;   // [1]
@@ -118,15 +157,16 @@ tc_score_kernel(const __grid_constant__ CUtensorMap tm_users, const __grid_const
     if (elect_one()) {
       tma_prefetch_desc(&tm_users);
       tma_prefetch_desc(&tm_items);
-      mbar_arrive_expect_tx(bar_users, TC_USER_BYTES);
-      for (int c = 0; c < 2; ++c) tma_load_2d(sm + TcSmem::users_off + c * 16384, &tm_users, bar_users, c * 32, q0);
-      for (int t = 0; t < n_tiles; ++t) {
-        const int s = t % TC_STAGES;
-        const uint32_t ph = (t / TC_STAGES) & 1;
+      mbar_arrive_expect_tx(bar_users, Sh::USER_BYTES);
+      for (int c = 0; c < Sh::KC; ++c) tma_load_2d(sm + Sm::users_off + c * 16384, &tm_users, bar_users, c * 32, q0);
+      for (int n = 0; n < n_tiles * Sh::SPT; ++n) {  // ring stage n: tile n / SPT, k-chunks (n % SPT) * SC ...
+        const int s = n % TC_STAGES;
+        const uint32_t ph = (n / TC_STAGES) & 1;
         mbar_wait(bar_empty + s, ph ^ 1);  // first pass through the ring passes immediately
-        mbar_arrive_expect_tx(bar_full + s, TC_TILE_BYTES);
-        for (int c = 0; c < 2; ++c)
-          tma_load_2d(sm + TcSmem::items_off + s * TC_TILE_BYTES + c * 16384, &tm_items, bar_full + s, c * 32, t * TC_TN);
+        mbar_arrive_expect_tx(bar_full + s, Sh::STAGE_BYTES);
+        for (int c = 0; c < Sh::SC; ++c)
+          tma_load_2d(sm + Sm::items_off + s * Sh::STAGE_BYTES + c * 16384, &tm_items, bar_full + s, ((n % Sh::SPT) * Sh::SC + c) * 32,
+                      (n / Sh::SPT) * TC_TN);
       }
     }
     return;
@@ -140,9 +180,9 @@ tc_score_kernel(const __grid_constant__ CUtensorMap tm_users, const __grid_const
   const int q = q0 + row;
   const bool active = row < a.ub && q < a.n_q;
   const int tix = chalf * TC_UB + row;  // column in the candidate arrays
-  float* cs = reinterpret_cast<float*>(sm + TcSmem::cand_s_off);
-  int32_t* ci = reinterpret_cast<int32_t*>(sm + TcSmem::cand_i_off);
-  float* stg = reinterpret_cast<float*>(sm + TcSmem::stage_off) + wg * 64 * TC_SROW;
+  float* cs = reinterpret_cast<float*>(sm + Sm::cand_s_off);
+  int32_t* ci = reinterpret_cast<int32_t*>(sm + Sm::cand_i_off);
+  float* stg = reinterpret_cast<float*>(sm + Sm::stage_off) + wg * 64 * TC_SROW;
   constexpr int LS = 2 * TC_UB;  // candidate slot stride
   float thr = -INFINITY;
   int cnt = 0;
@@ -230,24 +270,28 @@ tc_score_kernel(const __grid_constant__ CUtensorMap tm_users, const __grid_const
       }
     }
   };
-  const uint32_t ua = smem_u32(sm + TcSmem::users_off + wg * 8192);
+  const uint32_t ua = smem_u32(sm + Sm::users_off + wg * 8192);
   const int w4 = warp & 3, g = lane >> 2, tq = lane & 3;
   mbar_wait(bar_users, 0);
   for (int t = 0; t < n_tiles; ++t) {
-    const int s = t % TC_STAGES;
-    mbar_wait(bar_full + s, (t / TC_STAGES) & 1);
     float acc[64];
-    const uint32_t ib = smem_u32(sm + TcSmem::items_off + s * TC_TILE_BYTES);
-    wgmma_fence();
 #pragma unroll
-    for (int c = 0; c < 2; ++c)
+    for (int p = 0; p < Sh::SPT; ++p) {
+      const int n = t * Sh::SPT + p;
+      const int s = n % TC_STAGES;
+      mbar_wait(bar_full + s, (n / TC_STAGES) & 1);
+      const uint32_t ib = smem_u32(sm + Sm::items_off + s * Sh::STAGE_BYTES);
+      wgmma_fence();
 #pragma unroll
-      for (int k = 0; k < 4; ++k)
-        wgmma_m64n128k8_tf32_ss(acc, make_smem_desc_k_sw128(ua + c * 16384 + k * 32), make_smem_desc_k_sw128(ib + c * 16384 + k * 32),
-                                (c | k) ? 1u : 0u);
-    wgmma_commit();
-    wgmma_wait<0>();
-    if (lt == 0) mbar_arrive(bar_empty + s);  // this warpgroup is done reading the stage
+      for (int c = 0; c < Sh::SC; ++c)
+#pragma unroll
+        for (int k = 0; k < 4; ++k)
+          wgmma_m64n128k8_tf32_ss(acc, make_smem_desc_k_sw128(ua + (p * Sh::SC + c) * 16384 + k * 32),
+                                  make_smem_desc_k_sw128(ib + c * 16384 + k * 32), (p | c | k) ? 1u : 0u);
+      wgmma_commit();
+      wgmma_wait<0>();
+      if (lt == 0) mbar_arrive(bar_empty + s);  // this warpgroup is done reading the stage
+    }
     named_bar_sync(1 + wg, 128);             // the previous tile's staged scores have been read
 #pragma unroll
     for (int j = 0; j < 64; j += 2) {
@@ -281,7 +325,7 @@ tc_score_kernel(const __grid_constant__ CUtensorMap tm_users, const __grid_const
 }
 
 struct RescoreArgs {
-  const float* ug;          // gathered user rows [n_q_pad][64]
+  const float* ug;          // gathered user rows [n_q_pad][D]
   const float* item_emb;
   const float* unorm;
   const unsigned int* bmax_bits;
@@ -299,6 +343,7 @@ struct RescoreArgs {
   int32_t* fb_users;        // their user ids
 };
 
+template <int D>
 __global__ void __launch_bounds__(256) tc_rescore_kernel(const RescoreArgs a) {
   const int lane = threadIdx.x & 31;
   const int q = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
@@ -306,7 +351,7 @@ __global__ void __launch_bounds__(256) tc_rescore_kernel(const RescoreArgs a) {
   const int cnt_a = a.cand_n[(size_t)q * 2], cnt_b = a.cand_n[(size_t)q * 2 + 1];
   const int K = a.k;
   const float bmax = __uint_as_float(*a.bmax_bits);
-  const float E = (1.0f / 512.0f + 1.0f / 65536.0f + 1.0f / 262144.0f) * a.unorm[q] * bmax;  // TF32 truncation + slot tags
+  const float E = TcShape<D>::E * a.unorm[q] * bmax;  // TF32 truncation + k-step accumulation + slot tags
   // ---- prune by approximate score before any exact work ----
   // Every exact score lies within E of its approximate score.  Let a_K be the K-th largest approximate score of the
   // candidates: K candidates have an exact score >= a_K - E, so one whose approximate score is below a_K - 2E is beaten
@@ -362,16 +407,16 @@ __global__ void __launch_bounds__(256) tc_rescore_kernel(const RescoreArgs a) {
     s[h] = -INFINITY;
     if (h == 1 && cnt <= 32) continue;  // warp-uniform
     if (mine[h]) id[h] = sv[c];
-    // exact score: the same fp32 fma chain over k = 0..63 as impl 1 and the oracle
+    // exact score: the same fp32 fma chain over k = 0..D-1 as impl 1 and the oracle
     if (mine[h]) {
-      const float* u = a.ug + (size_t)q * TC_D;
-      const float4* it = reinterpret_cast<const float4*>(a.item_emb + (size_t)id[h] * TC_D);
-      float4 iv[TC_D / 4];  // the whole row in flight at once: this kernel is bound by the latency of these gathers
+      const float* u = a.ug + (size_t)q * D;
+      const float4* it = reinterpret_cast<const float4*>(a.item_emb + (size_t)id[h] * D);
+      float4 iv[D / 4];  // the whole row in flight at once: this kernel is bound by the latency of these gathers
 #pragma unroll
-      for (int k4 = 0; k4 < TC_D / 4; ++k4) iv[k4] = __ldg(it + k4);
+      for (int k4 = 0; k4 < D / 4; ++k4) iv[k4] = __ldg(it + k4);
       float acc = 0.f;
 #pragma unroll
-      for (int k4 = 0; k4 < TC_D / 4; ++k4) {
+      for (int k4 = 0; k4 < D / 4; ++k4) {
         const float4 uv = *reinterpret_cast<const float4*>(u + k4 * 4);
         acc = fmaf(uv.x, iv[k4].x, acc);
         acc = fmaf(uv.y, iv[k4].y, acc);
@@ -463,7 +508,9 @@ static int tc_fb_cap(int n_items) {
   return (int)cap;
 }
 
-static TcWorkspace tc_carve(char* base, int n_q, int n_items) {
+// The gathered user table is carved last: it is the only part whose size depends on d, so the fallback counter sits
+// at the same offset for every width (srb_topk_fallback_count_offset takes no d).
+static TcWorkspace tc_carve(char* base, int n_q, int n_items, int d) {
   TcWorkspace w;
   const int64_t n_q_pad = ((int64_t)n_q + 255) / 256 * 256 + 256;
   int64_t off = 0;
@@ -472,7 +519,6 @@ static TcWorkspace tc_carve(char* base, int n_q, int n_items) {
     off += tc_align(b);
     return p;
   };
-  w.ug = (float*)take(n_q_pad * TC_D * 4);
   w.unorm = (float*)take(n_q_pad * 4);
   w.bmax = (unsigned int*)take(16);
   w.cand_s = (float*)take((int64_t)n_q * TC_CAND * 4);
@@ -484,6 +530,7 @@ static TcWorkspace tc_carve(char* base, int n_q, int n_items) {
   w.fb_users = (int32_t*)take((int64_t)n_q * 4);
   w.fb_cap = tc_fb_cap(n_items);
   w.fb_scratch = (float*)take((int64_t)w.fb_cap * n_items * 4);
+  w.ug = (float*)take(n_q_pad * d * 4);
   w.bytes = off;
   return w;
 }
@@ -491,22 +538,16 @@ static TcWorkspace tc_carve(char* base, int n_q, int n_items) {
 int score_topk_fallback(const srb_topk_desc* d, const int32_t* fb_users, const int32_t* fb_rows, const int32_t* fb_count,
                         float* scratch, int fb_cap, cudaStream_t st);  // score_topk.cu
 
-int score_topk_tc(const srb_topk_desc* d, cudaStream_t st) {
-  SRB_REQUIRE(d->d == TC_D, "topk impl 2 (tensor cores) supports d=64 only (got %d)", d->d);
+template <int D>
+static int launch_tc(const srb_topk_desc* d, const TcWorkspace& w, cudaStream_t st) {
   const int n_q = d->n_q;
-  const TcWorkspace need = tc_carve(nullptr, n_q, d->n_items);
-  SRB_REQUIRE(d->workspace && d->workspace_bytes >= need.bytes, "topk impl 2: workspace too small (%lld < %lld)",
-              (long long)d->workspace_bytes, (long long)need.bytes);
-  SRB_REQUIRE(((uintptr_t)d->workspace & 255) == 0, "topk impl 2: workspace must be 256-byte aligned");
-  SRB_REQUIRE(((uintptr_t)d->item_emb & 15) == 0, "topk impl 2: item_emb must be 16-byte aligned");
-  TcWorkspace w = tc_carve((char*)d->workspace, n_q, d->n_items);
   const int n_q_pad = (n_q + 255) / 256 * 256 + 256;
   SRB_TRY(check_cuda(cudaMemsetAsync(w.bmax, 0, 16, st), "tc memset"));
   SRB_TRY(check_cuda(cudaMemsetAsync(w.fb_count, 0, 16, st), "tc memset"));
   {
     const long long rows = (long long)n_q_pad + d->n_items;
-    tc_gather_kernel<<<(unsigned)((rows + 7) / 8), 256, 0, st>>>(d->user_emb, d->users, n_q, n_q_pad, w.ug, w.unorm, d->item_emb,
-                                                                d->n_items, w.bmax);
+    tc_gather_kernel<D><<<(unsigned)((rows + 7) / 8), 256, 0, st>>>(d->user_emb, d->users, n_q, n_q_pad, w.ug, w.unorm, d->item_emb,
+                                                                   d->n_items, w.bmax);
     SRB_TRY(post_launch("tc_gather_kernel"));
   }
   // users per CTA: one wave of SMs when the queries fit (n_q <= TC_UB x SMs), else TC_UB per CTA and several waves
@@ -518,8 +559,8 @@ int score_topk_tc(const srb_topk_desc* d, cudaStream_t st) {
   if (ub < 32) ub = 32;
   const int blocks = (n_q + ub - 1) / ub;
   CUtensorMap tm_users, tm_items;
-  SRB_REQUIRE(make_tmap_f32_rows(&tm_users, w.ug, (uint64_t)n_q_pad, TC_D, TC_UB) == 0, "topk impl 2: cuTensorMapEncodeTiled(users) failed");
-  SRB_REQUIRE(make_tmap_f32_rows(&tm_items, d->item_emb, (uint64_t)d->n_items, TC_D, TC_TN) == 0,
+  SRB_REQUIRE(make_tmap_f32_rows(&tm_users, w.ug, (uint64_t)n_q_pad, D, TC_UB) == 0, "topk impl 2: cuTensorMapEncodeTiled(users) failed");
+  SRB_REQUIRE(make_tmap_f32_rows(&tm_items, d->item_emb, (uint64_t)d->n_items, D, TC_TN) == 0,
               "topk impl 2: cuTensorMapEncodeTiled(items) failed");
   TcArgs a;
   a.users = d->users;
@@ -532,13 +573,13 @@ int score_topk_tc(const srb_topk_desc* d, cudaStream_t st) {
   a.cand_i = w.cand_i;
   a.cand_n = w.cand_n;
   a.cand_thr = w.cand_thr;
-  const size_t smem = TcSmem::total + 1024;
+  const size_t smem = TcSmem<D>::total + 1024;
   static bool attr_done = false;
   if (!attr_done) {
-    SRB_TRY(check_cuda(cudaFuncSetAttribute(tc_score_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem), "tc smem attr"));
+    SRB_TRY(check_cuda(cudaFuncSetAttribute(tc_score_kernel<D>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem), "tc smem attr"));
     attr_done = true;
   }
-  tc_score_kernel<<<blocks, TC_THREADS, smem, st>>>(tm_users, tm_items, a);
+  tc_score_kernel<D><<<blocks, TC_THREADS, smem, st>>>(tm_users, tm_items, a);
   SRB_TRY(post_launch("tc_score_kernel"));
   RescoreArgs r;
   r.ug = w.ug;
@@ -559,24 +600,35 @@ int score_topk_tc(const srb_topk_desc* d, cudaStream_t st) {
   r.fb_count = w.fb_count;
   r.fb_rows = w.fb_rows;
   r.fb_users = w.fb_users;
-  tc_rescore_kernel<<<(n_q + 7) / 8, 256, 0, st>>>(r);
+  tc_rescore_kernel<D><<<(n_q + 7) / 8, 256, 0, st>>>(r);
   SRB_TRY(post_launch("tc_rescore_kernel"));
   return score_topk_fallback(d, w.fb_users, w.fb_rows, w.fb_count, w.fb_scratch, w.fb_cap, st);
+}
+
+int score_topk_tc(const srb_topk_desc* d, cudaStream_t st) {
+  SRB_REQUIRE(d->d == 64 || d->d == 128, "topk impl 2 (tensor cores) supports d=64 and d=128 only (got %d)", d->d);
+  const int n_q = d->n_q;
+  const TcWorkspace need = tc_carve(nullptr, n_q, d->n_items, d->d);
+  SRB_REQUIRE(d->workspace && d->workspace_bytes >= need.bytes, "topk impl 2: workspace too small (%lld < %lld)",
+              (long long)d->workspace_bytes, (long long)need.bytes);
+  SRB_REQUIRE(((uintptr_t)d->workspace & 255) == 0, "topk impl 2: workspace must be 256-byte aligned");
+  SRB_REQUIRE(((uintptr_t)d->item_emb & 15) == 0, "topk impl 2: item_emb must be 16-byte aligned");
+  const TcWorkspace w = tc_carve((char*)d->workspace, n_q, d->n_items, d->d);
+  return d->d == 64 ? launch_tc<64>(d, w, st) : launch_tc<128>(d, w, st);
 }
 
 }  // namespace srb
 
 // byte offset of the int32 fallback counter inside the workspace (diagnostics: how many users the
-// exact kernel had to re-run)
+// exact kernel had to re-run); the same for every width
 extern "C" int64_t srb_topk_fallback_count_offset(int32_t n_q, int32_t n_items) {
   if (n_q <= 0 || n_items <= 0) return -1;
-  const srb::TcWorkspace w = srb::tc_carve((char*)256, n_q, n_items);
+  const srb::TcWorkspace w = srb::tc_carve((char*)256, n_q, n_items, 64);
   return (int64_t)((char*)w.fb_count - (char*)256);
 }
 
 extern "C" int64_t srb_topk_workspace_bytes(int32_t n_q, int32_t n_items, int32_t d, int32_t k) {
-  (void)d;
   (void)k;
-  if (n_q <= 0 || n_items <= 0) return 0;
-  return srb::tc_carve(nullptr, n_q, n_items).bytes;
+  if (n_q <= 0 || n_items <= 0 || d <= 0) return 0;
+  return srb::tc_carve(nullptr, n_q, n_items, d).bytes;
 }

@@ -518,8 +518,8 @@ def score_topk(user_emb, item_emb, users, rated_ptr, rated_idx, k, impl=0, stats
     if rated_ptr is not None:
         rated_ptr, rated_idx = _i32(rated_ptr, dev), _i32(rated_idx, dev)
         desc.rated_ptr, desc.rated_idx = _p(rated_ptr), _p(rated_idx)
-    if impl == 0:  # auto: tensor-core path for the embedding size it is written for, else the CUDA-core kernel
-        impl = 2 if (d == 64 and item_emb.shape[0] >= 1024) else 1
+    if impl == 0:  # auto: tensor-core path for the embedding sizes it is written for, else the CUDA-core kernel
+        impl = 2 if (d in (64, 128) and item_emb.shape[0] >= 1024) else 1
     desc.k, desc.out_ids, desc.out_scores, desc.impl = k, _p(out_ids), _p(out_sc), impl
     ws = None
     if impl == 2:
