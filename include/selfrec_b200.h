@@ -314,7 +314,8 @@ int srb_adam_step(float* p, float* m, float* v, const float* g, int64_t n,
  *   out_ids  [n_q, k] int32, out_scores [n_q, k] fp32, score-descending
  * Selection follows find_k_largest's sequential semantics (strict > threshold, evict the
  * lexicographically smallest (score, id)); scores are exact fp32 fma chains over d.
- * k <= 32 in this version.
+ * k: 1..32 on impl 1; 1..256 on impl 2 (d = 64 or 128).  Longer lists, and lists over 32 at other
+ * widths, are extracted 32 at a time from dense score rows (selfrec_b200/ops.py _score_topk_wide).
  * ------------------------------------------------------------------------------------- */
 typedef struct srb_topk_desc {
   const float* user_emb;
@@ -329,9 +330,12 @@ typedef struct srb_topk_desc {
   int32_t* out_ids;
   float* out_scores;
   int32_t impl; /* 0 auto (impl 2 when d is 64 or 128, n_items >= 1024 and a workspace is given, else impl 1);
-                   1 CUDA cores, exact fp32; 2 (d = 64 or 128) wgmma TF32 candidate lists (2 x 24 per user) + exact fp32
-                   rescoring + a per-user exactness certificate, uncertified users re-run by the exact path */
-  void* workspace; /* impl 2: srb_topk_workspace_bytes(n_q, n_items, d, k) bytes, 256-byte aligned */
+                   1 CUDA cores, exact fp32, k <= 32 (k > 32 is refused);
+                   2 (d = 64 or 128, k <= 256) wgmma TF32 candidates + exact fp32 rescoring + a per-user exactness
+                   certificate, uncertified users re-run by the exact path.  k <= 32: candidate lists of 2 x 24 per
+                   user; 33 <= k <= 256: per-half candidate buffers behind a running threshold (DESIGN 4.4) */
+  void* workspace; /* impl 2: srb_topk_workspace_bytes(n_q, n_items, d, k) bytes, 256-byte aligned;
+                      O(n_q * k + n_items), never a dense [n_q, n_items] buffer */
   int64_t workspace_bytes;
 } srb_topk_desc;
 
@@ -438,7 +442,8 @@ int srb_graph_assemble(const srb_graph_assemble_desc* desc, void* stream);
 
 /* ---------------------------------------------------------------------------------------
  * Ranking metrics, device part (SURVEY 8(f) row 2; util/evaluation.py:9-15 `hits`, :85-97 NDCG):
- * hit_mask[q] bit r = 1 iff topk_ids[q, r] is in the test set of users[q]  (r < k <= 64).
+ * hit_mask[q * W + r / 64] bit r % 64 = 1 iff topk_ids[q, r] is in the test set of users[q]
+ * (r < k <= 256, W = ceil(k / 64) words per row: one word for k <= 64).
  * test_ptr / test_idx: CSR over user ids of the test items that have a training id, sorted per
  * user.  Hit Ratio / Precision / Recall / NDCG follow on the host from the masks with the
  * reference's own float expressions (selfrec_b200/util/evaluation.py), so they match bit for bit.

@@ -135,12 +135,13 @@ class GraphRecommender(Recommender):
 
     def _fast_measure(self):
         """fast_evaluation's metrics without leaving id space: full-catalog top-k on the device, hit masks on
-        the device (srb_rank_hit_masks), the reference's float expressions on the masks.  Same strings as
+        the device (srb_rank_hit_masks, ceil(max_N / 64) words per user), the reference's float expressions on the
+        masks, for max_N <= 256.  Same strings as
         ranking_evaluation(self.data.test_set, self.test(), [self.max_N])."""
         data = self.data
         names = list(data.test_set)
         ranker = self.shard_ranker
-        if not ((ranker is not None or self._has_embedding_tables()) and self.max_N <= 64 and all(u in data.user for u in names)):
+        if not ((ranker is not None or self._has_embedding_tables()) and self.max_N <= ops.TOPK_TC_MAX and all(u in data.user for u in names)):
             return ranking_evaluation(data.test_set, self.test(), [self.max_N])
         uids = np.fromiter((data.user[u] for u in names), dtype=np.int32, count=len(names))
         test_ptr, test_idx, n_test = data.test_csr()

@@ -319,9 +319,154 @@ __global__ void __launch_bounds__(256) fb_topk_kernel(const float* scratch, cons
   }
 }
 
+// Long lists (k > 32): one CTA per uncertified user at a time, at most `cap` users in flight (one scratch row each).
+// The CTA writes the user's exact masked row, finds the k-th largest score s* by a 4-pass 8-bit radix select, keeps
+// every score above it and, of the scores equal to it, find_k_largest's choice: among those within the first k items
+// (in id order) scoring >= s* -- the ones that entered the list -- the largest ids, as many as the list has room for
+// (tc_rescore_long_kernel states the rule), and writes the list score-descending, ties by id descending.
+__device__ __forceinline__ uint32_t fb_okey(float s) {  // order-preserving float -> uint32 (+0 and -0 alike)
+  const uint32_t b = __float_as_uint(s == 0.f ? 0.f : s);
+  return (b & 0x80000000u) ? ~b : (b | 0x80000000u);
+}
+
+template <int D>
+__global__ void __launch_bounds__(256, 1) fb_long_kernel(const float* __restrict__ user_emb, const float* __restrict__ item_emb,
+                                                     const int32_t* __restrict__ fb_users, const int32_t* __restrict__ fb_rows,
+                                                     const int32_t* __restrict__ fb_count, const int32_t* __restrict__ rated_ptr,
+                                                     const int32_t* __restrict__ rated_idx, int n_items, int k, float* scratch,
+                                                     int32_t* out_ids, float* out_scores) {
+  __shared__ float us[D];
+  __shared__ int hist[256];
+  __shared__ float sel_s[256];
+  __shared__ int32_t sel_i[256];
+  __shared__ int32_t tie_i[256];  // tied items that entered the list, in id order
+  __shared__ int wsum[8];
+  __shared__ int s_need, s_nsel, s_ent;
+  __shared__ uint32_t s_pref;
+  const int tid = threadIdx.x, lane = tid & 31, wid = tid >> 5;
+  const int count = *fb_count;
+  float* row = scratch + (size_t)blockIdx.x * n_items;
+  for (int slot = blockIdx.x; slot < count; slot += gridDim.x) {
+    const int u = fb_users[slot];
+    __syncthreads();
+    for (int kk = tid; kk < D; kk += 256) us[kk] = user_emb[(size_t)u * D + kk];
+    __syncthreads();
+    for (int i = tid; i < n_items; i += 256) {  // the fma chain and the mask of fb_score_kernel
+      const float* it = item_emb + (size_t)i * D;
+      float acc = 0.f;
+#pragma unroll 8
+      for (int k4 = 0; k4 < D / 4; ++k4) {
+        const float4 v = ldg4(it + k4 * 4);
+        acc = fmaf(us[k4 * 4 + 0], v.x, acc);
+        acc = fmaf(us[k4 * 4 + 1], v.y, acc);
+        acc = fmaf(us[k4 * 4 + 2], v.z, acc);
+        acc = fmaf(us[k4 * 4 + 3], v.w, acc);
+      }
+      if (rated_ptr) {
+        int lo = rated_ptr[u], hi = rated_ptr[u + 1];
+        while (lo < hi) {
+          const int mid = (lo + hi) >> 1;
+          if (rated_idx[mid] < i) lo = mid + 1; else hi = mid;
+        }
+        if (lo < rated_ptr[u + 1] && rated_idx[lo] == i) acc = TK_MASKED;
+      }
+      row[i] = acc;
+    }
+    __syncthreads();
+    // radix select of the k-th largest key: pref = its key, need = how many of the entries equal to it to keep
+    uint32_t pref = 0, pmask = 0;
+    int need = k;
+    for (int shift = 24; shift >= 0; shift -= 8) {
+      hist[tid] = 0;
+      __syncthreads();
+      for (int i = tid; i < n_items; i += 256) {
+        const uint32_t key = fb_okey(row[i]);
+        if ((key & pmask) == pref) atomicAdd(&hist[(key >> shift) & 255], 1);
+      }
+      __syncthreads();
+      if (tid == 0) {
+        int cum = 0, b = 255;
+        for (; b > 0 && cum + hist[b] < need; --b) cum += hist[b];
+        s_need = need - cum;
+        s_pref = pref | ((uint32_t)b << shift);
+        s_nsel = 0;
+      }
+      __syncthreads();
+      need = s_need;
+      pref = s_pref;
+      pmask |= 0xffu << shift;
+    }
+    // above the k-th: any slot of the first k - need; equal to it: the `need` smallest ids, visited in id order
+    for (int i = tid; i < n_items; i += 256) {
+      const float sc = row[i];
+      if (fb_okey(sc) > pref) {
+        const int p = atomicAdd(&s_nsel, 1);
+        sel_s[p] = sc;
+        sel_i[p] = i;
+      }
+    }
+    // walk the items in id order until k of them score >= s*; the tied ones among them entered
+    int seen = 0, ties = 0;
+    if (tid == 0) s_ent = 0;
+    __syncthreads();
+    for (int base = 0; base < n_items && seen < k; base += 256) {
+      const int i = base + tid;
+      const uint32_t key = i < n_items ? fb_okey(row[i]) : 0u;
+      const bool ge = i < n_items && key >= pref, tie = i < n_items && key == pref;
+      const unsigned bg = __ballot_sync(SRB_FULL_MASK, ge), bt = __ballot_sync(SRB_FULL_MASK, tie);
+      if (lane == 0) wsum[wid] = __popc(bg) | (__popc(bt) << 16);
+      __syncthreads();
+      int og = 0, ot = 0, tg = 0, tt = 0;
+#pragma unroll
+      for (int w = 0; w < 8; ++w) {
+        const int v = wsum[w];
+        og += (w < wid) ? (v & 0xffff) : 0;
+        ot += (w < wid) ? (v >> 16) : 0;
+        tg += v & 0xffff;
+        tt += v >> 16;
+      }
+      const unsigned lt = (1u << lane) - 1u;
+      if (tie && seen + og + __popc(bg & lt) < k) {  // entered: the entered ties are a prefix of the ties
+        const int t = ties + ot + __popc(bt & lt);
+        tie_i[t] = i;
+        atomicMax(&s_ent, t + 1);
+      }
+      seen += tg;
+      ties += tt;
+      __syncthreads();
+    }
+    ties = s_ent;
+    for (int t = tid; t < k; t += 256) {
+      if (t >= k - need) {  // the largest `need` ids of the entered ties
+        const int i = tie_i[ties - (k - t)];
+        sel_s[t] = row[i];
+        sel_i[t] = i;
+      }
+    }
+    __syncthreads();
+    const size_t orow = (size_t)fb_rows[slot];
+    for (int p = tid; p < k; p += 256) {
+      const uint32_t ek = fb_okey(sel_s[p]);
+      const int id = sel_i[p];
+      int pos = 0;
+      for (int j = 0; j < k; ++j) {
+        const uint32_t oj = fb_okey(sel_s[j]);
+        pos += (oj > ek) || (oj == ek && sel_i[j] > id);
+      }
+      out_ids[orow * k + pos] = id;
+      out_scores[orow * k + pos] = sel_s[p];
+    }
+  }
+}
+
 template <int D>
 static int score_topk_fallback_d(const srb_topk_desc* d, const int32_t* fb_users, const int32_t* fb_rows, const int32_t* fb_count,
                                  float* scratch, int fb_cap, cudaStream_t st) {
+  if (d->k > 32) {  // long lists: every uncertified user, fb_cap at a time
+    fb_long_kernel<D><<<fb_cap, 256, 0, st>>>(d->user_emb, d->item_emb, fb_users, fb_rows, fb_count, d->rated_ptr, d->rated_idx,
+                                              d->n_items, d->k, scratch, d->out_ids, d->out_scores);
+    return post_launch("fb_long_kernel");
+  }
   // fast path: up to fb_cap users
   dim3 grid((d->n_items + 255) / 256, fb_cap < 8 ? fb_cap : 8);
   fb_score_kernel<D><<<grid, 256, 0, st>>>(d->user_emb, d->item_emb, fb_users, fb_count, d->rated_ptr, d->rated_idx, d->n_items,
@@ -362,12 +507,14 @@ extern "C" int srb_score_topk(const srb_topk_desc* d, void* stream) {
   if (d->n_q == 0) return SRB_OK;  // empty query list: nothing to launch (pointers may be null)
   SRB_REQUIRE(d->user_emb && d->item_emb && d->users && d->out_ids && d->out_scores, "topk: null pointer");
   SRB_REQUIRE((d->rated_ptr == nullptr) == (d->rated_idx == nullptr), "topk: rated_ptr/rated_idx must both be set or both null");
-  SRB_REQUIRE(d->k >= 1 && d->k <= 32, "topk: k=%d unsupported (1..32)", d->k);
   SRB_REQUIRE(d->n_items >= 1 && d->n_q >= 0, "topk: bad shape");
   SRB_REQUIRE(d->impl >= 0 && d->impl <= 2, "topk: bad impl");
   if (d->n_q == 0) return SRB_OK;
-  if (d->impl == 2 || (d->impl == 0 && (d->d == 64 || d->d == 128) && d->workspace != nullptr && d->n_items >= 1024))
-    return srb::score_topk_tc(d, (cudaStream_t)stream);
+  const bool tc = d->impl == 2 || (d->impl == 0 && (d->d == 64 || d->d == 128) && d->workspace != nullptr && d->n_items >= 1024);
+  // impl 1 keeps one list entry per lane (k <= 32); impl 2 also takes the long lists (k <= 256)
+  SRB_REQUIRE(d->k >= 1 && d->k <= (tc ? 256 : 32), "topk: k=%d unsupported (1..32; impl 2 at d = 64/128: 1..256)", d->k);
+  SRB_REQUIRE(d->k <= 32 || d->k <= d->n_items, "topk: k=%d exceeds n_items=%d", d->k, d->n_items);
+  if (tc) return srb::score_topk_tc(d, (cudaStream_t)stream);
   srb::TopkArgs a;
   a.user_emb = d->user_emb;
   a.item_emb = d->item_emb;
@@ -421,7 +568,8 @@ extern "C" int srb_score_rows(const float* user_emb, const float* item_emb, int3
 }
 
 namespace srb {
-// one warp per query row: lane r (and r + 32) looks its recommended id up in the user's sorted test list
+// one warp per query row: lane r (and r + 32, ...) looks its recommended id up in the user's sorted test list;
+// ceil(k / 64) words per row, bit r % 64 of word r / 64 for rank r
 __global__ void __launch_bounds__(256) rank_hit_masks_kernel(const int32_t* __restrict__ ids, int n_q, int k, const int32_t* __restrict__ users,
                                                              const int32_t* __restrict__ test_ptr, const int32_t* __restrict__ test_idx,
                                                              unsigned long long* __restrict__ out) {
@@ -430,9 +578,11 @@ __global__ void __launch_bounds__(256) rank_hit_masks_kernel(const int32_t* __re
   if (q >= n_q) return;
   const int u = users[q];
   const int beg = test_ptr[u], end = test_ptr[u + 1];
+  const int words = (k + 63) / 64;
+  for (int wd = 0; wd < words; ++wd) {
   unsigned long long mask = 0;
   for (int half = 0; half < 2; ++half) {
-    const int r = half * 32 + lane;
+    const int r = wd * 64 + half * 32 + lane;
     bool hit = false;
     if (r < k) {
       const int id = ids[(size_t)q * k + r];
@@ -446,13 +596,14 @@ __global__ void __launch_bounds__(256) rank_hit_masks_kernel(const int32_t* __re
     }
     mask |= (unsigned long long)__ballot_sync(SRB_FULL_MASK, hit) << (32 * half);
   }
-  if (lane == 0) out[q] = mask;
+  if (lane == 0) out[(size_t)q * words + wd] = mask;
+  }
 }
 }  // namespace srb
 
 extern "C" int srb_rank_hit_masks(const int32_t* topk_ids, int32_t n_q, int32_t k, const int32_t* users, const int32_t* test_ptr,
                                   const int32_t* test_idx, uint64_t* hit_mask, void* stream) {
-  SRB_REQUIRE(n_q >= 0 && k >= 1 && k <= 64, "rank_hit_masks: k must be 1..64");
+  SRB_REQUIRE(n_q >= 0 && k >= 1 && k <= 256, "rank_hit_masks: k must be 1..256");
   if (n_q == 0) return SRB_OK;
   SRB_REQUIRE(topk_ids && users && test_ptr && test_idx && hit_mask, "rank_hit_masks: null pointer");
   srb::rank_hit_masks_kernel<<<(n_q + 7) / 8, 256, 0, (cudaStream_t)stream>>>(topk_ids, n_q, k, users, test_ptr, test_idx,

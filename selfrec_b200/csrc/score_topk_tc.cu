@@ -25,6 +25,9 @@
 //                               half has approx score <= that half's 24th best, so the result is exact iff
 //                               thr32 := max of the two + E(D) < exact k-th score.  Users failing it (or with fewer than
 //                               k unrated items) are re-run by the exact CUDA-core kernel (impl 1).
+// Lists of 33..256 (tc_score_kernel<D, true>): the select keeps, per user row x column half, a candidate buffer in global
+// memory behind a running threshold instead of the 24-slot list; tc_rescore_long_kernel (CTA per user) rescoring and
+// certifying them, fb_long_kernel (score_topk.cu) re-running the uncertified users (DESIGN 4.4).
 #include "common.cuh"
 #include "tc_common.cuh"
 
@@ -84,7 +87,29 @@ struct TcArgs {
   int32_t* cand_i;           // [n_q][2][24]
   int32_t* cand_n;           // [n_q][2]
   float* cand_thr;           // [n_q][2] min approx score of a full list, else -inf
+  // long lists (k > 32, tc_score_kernel<D, true>): per column half a candidate buffer of `cap` (score, id) slots
+  // behind a running threshold instead of the 24-slot list (DESIGN 4.4)
+  int32_t k;
+  int32_t cap;
+  float* buf_s;              // [n_q][2][cap] approx scores
+  int32_t* buf_i;            // [n_q][2][cap]
+  const float* unorm;        // ||u_q|| and max ||item|| (tc_gather_kernel): the error bound E of the threshold
+  const unsigned int* bmax_bits;
 };
+
+constexpr int TC_LONG_MAX = 256;  // longest list of the long-list route
+
+// per-half candidate capacity of a long list of k: room for the k best, the 2E band below them and a refill
+static int tc_long_cap(int k) { return (2 * k + 256 + 31) / 32 * 32; }
+
+// order-preserving map of a float to uint32 (+0 and -0 map alike) and back
+__device__ __forceinline__ uint32_t tc_okey(float s) {
+  const uint32_t b = __float_as_uint(s == 0.f ? 0.f : s);
+  return (b & 0x80000000u) ? ~b : (b | 0x80000000u);
+}
+__device__ __forceinline__ float tc_ofloat(uint32_t key) {
+  return __uint_as_float((key & 0x80000000u) ? (key & 0x7fffffffu) : ~key);
+}
 
 template <int D>
 struct TcVec;  // the D/32 floats of a row that one lane gathers
@@ -126,7 +151,7 @@ __global__ void __launch_bounds__(256) tc_gather_kernel(const float* __restrict_
   }
 }
 
-template <int D>
+template <int D, bool LONG>
 __global__ void __launch_bounds__(TC_THREADS, 1)
 tc_score_kernel(const __grid_constant__ CUtensorMap tm_users, const __grid_constant__ CUtensorMap tm_items, const TcArgs a) {
   extern __shared__ __align__(1024) uint8_t tc_smem_raw[];
@@ -203,6 +228,45 @@ tc_score_kernel(const __grid_constant__ CUtensorMap tm_users, const __grid_const
   // the certificate in tc_rescore_kernel accounts for the 2^-20 relative perturbation), so a bucket's minimum
   // names its own slot and 7 FMNMX replace a compare/select scan.
   float bm0 = INFINITY, bm1 = INFINITY, bm2 = INFINITY;  // bucket minima (valid once full)
+  // long lists: thr is a running threshold; every unrated item of the half with approx score > thr is appended to the
+  // half's buffer.  A full buffer is compacted: thr rises to (a lower bound of the k-th best approx score in the
+  // buffer) - 2E and entries <= thr are dropped.  thr only rises, so at the end every item above the final thr is in
+  // the buffer.  A compaction that frees less than a quarter of it (a band of near-ties wider than the buffer) marks
+  // the half uncertified: cnt = -1, thr = +inf.
+  float* bs = nullptr;
+  int32_t* bi = nullptr;
+  float twoE = 0.f;
+  if constexpr (LONG) {
+    if (active) {
+      bs = a.buf_s + ((size_t)q * 2 + chalf) * a.cap;
+      bi = a.buf_i + ((size_t)q * 2 + chalf) * a.cap;
+      twoE = 2.0f * Sh::E * a.unorm[q] * __uint_as_float(*a.bmax_bits);
+    }
+  }
+  auto compact = [&]() {
+    // largest key v with 12 low zero bits such that >= k buffered scores have key >= v: v <= the k-th best key
+    uint32_t v = 0;
+    for (int b = 31; b >= 12; --b) {
+      const uint32_t t = v | (1u << b);
+      int c = 0;
+      for (int p = 0; p < a.cap; ++p) c += tc_okey(bs[p]) >= t;
+      if (c >= a.k) v = t;
+    }
+    if (v != 0) thr = fmaxf(thr, tc_ofloat(v) - twoE);
+    int kept = 0;
+    for (int p = 0; p < a.cap; ++p) {
+      const float s = bs[p];
+      if (s > thr) {
+        bi[kept] = bi[p];
+        bs[kept++] = s;
+      }
+    }
+    cnt = kept;
+    if (kept > a.cap - a.cap / 4) {
+      cnt = -1;
+      thr = INFINITY;
+    }
+  };
   auto process_group = [&](const uint32_t (&r)[32], int g0) {
     uint32_t mask = 0;
 #pragma unroll
@@ -234,6 +298,12 @@ tc_score_kernel(const __grid_constant__ CUtensorMap tm_users, const __grid_const
       float sc = __uint_as_float((j & 16) ? t2b : t2a);
       if (!(sc > thr)) continue;  // thr may have risen inside this group
       const int id = g0 + j;
+      if constexpr (LONG) {
+        bs[cnt] = sc;
+        bi[cnt] = id;
+        if (++cnt == a.cap) compact();
+        continue;
+      }
       if (cnt < TC_LIST) {
         cs[cnt * LS + tix] = sc;
         ci[cnt * LS + tix] = id;
@@ -313,6 +383,13 @@ tc_score_kernel(const __grid_constant__ CUtensorMap tm_users, const __grid_const
       process_group(r, c0 + h * 32);
     }
   }
+  if constexpr (LONG) {
+    if (active) {
+      a.cand_n[(size_t)q * 2 + chalf] = cnt;
+      a.cand_thr[(size_t)q * 2 + chalf] = thr;
+    }
+    return;
+  }
   if (active) {
     const size_t o = ((size_t)q * 2 + chalf) * TC_LIST;
     for (int p = 0; p < TC_LIST; ++p) {
@@ -341,6 +418,9 @@ struct RescoreArgs {
   int32_t* fb_count;        // device counter of users needing the exact fallback
   int32_t* fb_rows;         // their query rows
   int32_t* fb_users;        // their user ids
+  int32_t cap;              // long lists: per-half buffer capacity and the buffers of tc_score_kernel<D, true>
+  const float* buf_s;
+  const int32_t* buf_i;
 };
 
 template <int D>
@@ -483,6 +563,158 @@ __global__ void __launch_bounds__(256) tc_rescore_kernel(const RescoreArgs a) {
   }
 }
 
+// sum over the 256 threads of a block (every thread gets it); red: 8 ints of shared memory
+__device__ __forceinline__ int tc_block_sum(int v, int* red) {
+  v = warp_sum(v);
+  __syncthreads();  // red is free again (its previous use has been read)
+  if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = v;
+  __syncthreads();
+  int s = 0;
+#pragma unroll
+  for (int w = 0; w < 8; ++w) s += red[w];
+  return s;
+}
+
+constexpr int TC_LONG_CAND = 2 * ((2 * TC_LONG_MAX + 256 + 31) / 32 * 32);  // both halves' buffers at k = 256
+
+// Long lists (k > 32): CTA per user over the candidates of both half buffers.  The same approximate prune as
+// tc_rescore_kernel (a_K - 2E), exact fp32 fma-chain scores of the survivors, then the set find_k_largest keeps when it
+// visits the items in id order, written score-descending, ties by id descending.  With s* the k-th score, that set is
+// every score above s* and, of the scores equal to s*, those among the first k items (in id order) scoring >= s* --
+// the ones that found the list not yet full at s* and entered -- minus the smallest ids, which the later, greater
+// scores evicted first: the largest (k - #above) ids of them.
+// Certificate: every item outside the buffers has approx score <= thr (the larger of the two halves' final running
+// thresholds), so the list is exact iff thr + E < the exact k-th score; otherwise, or when a buffer overflowed or
+// the user has fewer than k unrated items, the user goes to the exact fallback.
+template <int D>
+__global__ void __launch_bounds__(256) tc_rescore_long_kernel(const RescoreArgs a) {
+  __shared__ float s_ap[TC_LONG_CAND];       // approx scores, then the survivors' exact-score keys
+  __shared__ int32_t s_id[TC_LONG_CAND];
+  __shared__ int32_t s_sv[TC_LONG_CAND];     // survivor ids
+  __shared__ int32_t s_rank[TC_LONG_CAND];   // per survivor: 2 above s*, 1 tied with s* and entered, 0 otherwise
+  __shared__ int red[8];
+  __shared__ int s_cnt;
+  __shared__ float s_kth;
+  __shared__ uint32_t s_kkey;
+  const int q = blockIdx.x;
+  const int tid = threadIdx.x;
+  const int K = a.k;
+  const int n0 = a.cand_n[(size_t)q * 2], n1 = a.cand_n[(size_t)q * 2 + 1];
+  int deg = 0;
+  if (a.rated_ptr) {
+    const int u = a.users[q];
+    deg = a.rated_ptr[u + 1] - a.rated_ptr[u];
+  }
+  const float E = TcShape<D>::E * a.unorm[q] * __uint_as_float(*a.bmax_bits);
+  bool unsafe = n0 < 0 || n1 < 0 || n0 + n1 < K || a.n_items - deg < K;
+  if (!unsafe) {
+    const int n = n0 + n1;
+    for (int c = tid; c < n; c += 256) {
+      const size_t o = (c < n0) ? (size_t)q * 2 * a.cap + c : ((size_t)q * 2 + 1) * a.cap + (c - n0);
+      s_ap[c] = a.buf_s[o];
+      s_id[c] = a.buf_i[o];
+    }
+    if (tid == 0) s_cnt = 0;
+    __syncthreads();
+    // the K-th largest approximate key, bit by bit
+    uint32_t v = 0;
+    for (int b = 31; b >= 0; --b) {
+      const uint32_t t = v | (1u << b);
+      int c = 0;
+      for (int p = tid; p < n; p += 256) c += tc_okey(s_ap[p]) >= t;
+      if (tc_block_sum(c, red) >= K) v = t;
+    }
+    const float cut = tc_ofloat(v) - 2.0f * E;
+    for (int p = tid; p < n; p += 256)
+      if (s_ap[p] >= cut) s_sv[atomicAdd(&s_cnt, 1)] = s_id[p];
+    __syncthreads();
+    const int S = s_cnt;
+    // exact score: the same fp32 fma chain over k = 0..D-1 as impl 1 and the oracle
+    uint32_t* s_ek = reinterpret_cast<uint32_t*>(s_ap);
+    const float* u = a.ug + (size_t)q * D;
+    for (int p = tid; p < S; p += 256) {
+      const float4* it = reinterpret_cast<const float4*>(a.item_emb + (size_t)s_sv[p] * D);
+      float acc = 0.f;
+#pragma unroll 8
+      for (int k4 = 0; k4 < D / 4; ++k4) {
+        const float4 uv = *reinterpret_cast<const float4*>(u + k4 * 4);
+        const float4 iv = __ldg(it + k4);
+        acc = fmaf(uv.x, iv.x, acc);
+        acc = fmaf(uv.y, iv.y, acc);
+        acc = fmaf(uv.z, iv.z, acc);
+        acc = fmaf(uv.w, iv.w, acc);
+      }
+      s_ek[p] = tc_okey(acc);
+    }
+    __syncthreads();
+    for (int p = tid; p < S; p += 256) {
+      const uint32_t ek = s_ek[p];
+      const int id = s_sv[p];
+      int r = 0;
+      for (int j = 0; j < S; ++j) {
+        const uint32_t oj = s_ek[j];
+        r += (oj > ek) || (oj == ek && s_sv[j] < id);
+      }
+      if (r == K - 1) {
+        s_kth = tc_ofloat(ek);
+        s_kkey = ek;
+      }
+    }
+    __syncthreads();
+    const float thr = fmaxf(a.cand_thr[(size_t)q * 2], a.cand_thr[(size_t)q * 2 + 1]);
+    unsafe = !(thr + E < s_kth);
+    if (!unsafe) {
+      const uint32_t kk = s_kkey;
+      int above = 0;
+      for (int p = tid; p < S; p += 256) {
+        const uint32_t ek = s_ek[p];
+        int st = 0;
+        if (ek > kk) {
+          st = 2;
+          ++above;
+        } else if (ek == kk) {  // entered iff fewer than k scores >= s* precede it in id order
+          const int id = s_sv[p];
+          int before = 0;
+          for (int j = 0; j < S; ++j) before += s_ek[j] >= kk && s_sv[j] < id;
+          st = before < K ? 1 : 0;
+        }
+        s_rank[p] = st;
+      }
+      const int need = K - tc_block_sum(above, red);  // also orders the s_rank writes before the reads below
+      int32_t* keep = s_id;                            // free since the survivors were listed
+      for (int p = tid; p < S; p += 256) {
+        int k_ = s_rank[p] == 2;
+        if (s_rank[p] == 1) {
+          const int id = s_sv[p];
+          int larger = 0;
+          for (int j = 0; j < S; ++j) larger += s_rank[j] == 1 && s_sv[j] > id;
+          k_ = larger < need;
+        }
+        keep[p] = k_;
+      }
+      __syncthreads();
+      for (int p = tid; p < S; p += 256) {
+        if (!keep[p]) continue;
+        const uint32_t ek = s_ek[p];
+        const int id = s_sv[p];
+        int pos = 0;
+        for (int j = 0; j < S; ++j) {
+          const uint32_t oj = s_ek[j];
+          pos += keep[j] && ((oj > ek) || (oj == ek && s_sv[j] > id));
+        }
+        a.out_ids[(size_t)q * K + pos] = id;
+        a.out_scores[(size_t)q * K + pos] = tc_ofloat(ek);
+      }
+      return;
+    }
+  }
+  if (tid == 0) {
+    const int slot = atomicAdd(a.fb_count, 1);
+    a.fb_rows[slot] = q;
+    a.fb_users[slot] = a.users[q];
+  }
+}
+
 static int64_t tc_align(int64_t x) { return (x + 255) / 256 * 256; }
 
 struct TcWorkspace {
@@ -498,6 +730,9 @@ struct TcWorkspace {
   int32_t* fb_users;
   float* fb_scratch;  // [fb_cap][n_items] exact score rows of the users re-run by the fast fallback
   int32_t fb_cap;
+  float* buf_s;       // long lists: [n_q][2][cap] candidate buffers (empty at k <= 32)
+  int32_t* buf_i;
+  int32_t cap;
   int64_t bytes;
 };
 
@@ -509,8 +744,9 @@ static int tc_fb_cap(int n_items) {
 }
 
 // The gathered user table is carved last: it is the only part whose size depends on d, so the fallback counter sits
-// at the same offset for every width (srb_topk_fallback_count_offset takes no d).
-static TcWorkspace tc_carve(char* base, int n_q, int n_items, int d) {
+// at the same offset for every width (srb_topk_fallback_count_offset takes no d).  The long-list buffers, the only
+// part whose size depends on k, come after the counter too; at k <= 32 they are empty and the layout is unchanged.
+static TcWorkspace tc_carve(char* base, int n_q, int n_items, int d, int k) {
   TcWorkspace w;
   const int64_t n_q_pad = ((int64_t)n_q + 255) / 256 * 256 + 256;
   int64_t off = 0;
@@ -530,6 +766,9 @@ static TcWorkspace tc_carve(char* base, int n_q, int n_items, int d) {
   w.fb_users = (int32_t*)take((int64_t)n_q * 4);
   w.fb_cap = tc_fb_cap(n_items);
   w.fb_scratch = (float*)take((int64_t)w.fb_cap * n_items * 4);
+  w.cap = (k > 32) ? tc_long_cap(k) : 0;
+  w.buf_s = (float*)take((int64_t)n_q * 2 * w.cap * 4);
+  w.buf_i = (int32_t*)take((int64_t)n_q * 2 * w.cap * 4);
   w.ug = (float*)take(n_q_pad * d * 4);
   w.bytes = off;
   return w;
@@ -537,6 +776,18 @@ static TcWorkspace tc_carve(char* base, int n_q, int n_items, int d) {
 
 int score_topk_fallback(const srb_topk_desc* d, const int32_t* fb_users, const int32_t* fb_rows, const int32_t* fb_count,
                         float* scratch, int fb_cap, cudaStream_t st);  // score_topk.cu
+
+template <int D, bool LONG>
+static int launch_tc_score(const CUtensorMap& tm_users, const CUtensorMap& tm_items, const TcArgs& a, int blocks, cudaStream_t st) {
+  const size_t smem = TcSmem<D>::total + 1024;
+  static bool attr_done = false;
+  if (!attr_done) {
+    SRB_TRY(check_cuda(cudaFuncSetAttribute(tc_score_kernel<D, LONG>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem), "tc smem attr"));
+    attr_done = true;
+  }
+  tc_score_kernel<D, LONG><<<blocks, TC_THREADS, smem, st>>>(tm_users, tm_items, a);
+  return post_launch("tc_score_kernel");
+}
 
 template <int D>
 static int launch_tc(const srb_topk_desc* d, const TcWorkspace& w, cudaStream_t st) {
@@ -573,14 +824,18 @@ static int launch_tc(const srb_topk_desc* d, const TcWorkspace& w, cudaStream_t 
   a.cand_i = w.cand_i;
   a.cand_n = w.cand_n;
   a.cand_thr = w.cand_thr;
-  const size_t smem = TcSmem<D>::total + 1024;
-  static bool attr_done = false;
-  if (!attr_done) {
-    SRB_TRY(check_cuda(cudaFuncSetAttribute(tc_score_kernel<D>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem), "tc smem attr"));
-    attr_done = true;
+  a.k = d->k;
+  a.cap = w.cap;
+  a.buf_s = w.buf_s;
+  a.buf_i = w.buf_i;
+  a.unorm = w.unorm;
+  a.bmax_bits = w.bmax;
+  const bool lng = d->k > 32;
+  if (lng) {
+    SRB_TRY((launch_tc_score<D, true>(tm_users, tm_items, a, blocks, st)));
+  } else {
+    SRB_TRY((launch_tc_score<D, false>(tm_users, tm_items, a, blocks, st)));
   }
-  tc_score_kernel<D><<<blocks, TC_THREADS, smem, st>>>(tm_users, tm_items, a);
-  SRB_TRY(post_launch("tc_score_kernel"));
   RescoreArgs r;
   r.ug = w.ug;
   r.item_emb = d->item_emb;
@@ -600,35 +855,44 @@ static int launch_tc(const srb_topk_desc* d, const TcWorkspace& w, cudaStream_t 
   r.fb_count = w.fb_count;
   r.fb_rows = w.fb_rows;
   r.fb_users = w.fb_users;
-  tc_rescore_kernel<D><<<(n_q + 7) / 8, 256, 0, st>>>(r);
-  SRB_TRY(post_launch("tc_rescore_kernel"));
+  r.cap = w.cap;
+  r.buf_s = w.buf_s;
+  r.buf_i = w.buf_i;
+  if (lng) {
+    tc_rescore_long_kernel<D><<<n_q, 256, 0, st>>>(r);
+    SRB_TRY(post_launch("tc_rescore_long_kernel"));
+  } else {
+    tc_rescore_kernel<D><<<(n_q + 7) / 8, 256, 0, st>>>(r);
+    SRB_TRY(post_launch("tc_rescore_kernel"));
+  }
   return score_topk_fallback(d, w.fb_users, w.fb_rows, w.fb_count, w.fb_scratch, w.fb_cap, st);
 }
 
 int score_topk_tc(const srb_topk_desc* d, cudaStream_t st) {
   SRB_REQUIRE(d->d == 64 || d->d == 128, "topk impl 2 (tensor cores) supports d=64 and d=128 only (got %d)", d->d);
+  SRB_REQUIRE(d->k >= 1 && d->k <= TC_LONG_MAX, "topk impl 2: k=%d unsupported (1..%d)", d->k, TC_LONG_MAX);
   const int n_q = d->n_q;
-  const TcWorkspace need = tc_carve(nullptr, n_q, d->n_items, d->d);
+  const TcWorkspace need = tc_carve(nullptr, n_q, d->n_items, d->d, d->k);
   SRB_REQUIRE(d->workspace && d->workspace_bytes >= need.bytes, "topk impl 2: workspace too small (%lld < %lld)",
               (long long)d->workspace_bytes, (long long)need.bytes);
   SRB_REQUIRE(((uintptr_t)d->workspace & 255) == 0, "topk impl 2: workspace must be 256-byte aligned");
   SRB_REQUIRE(((uintptr_t)d->item_emb & 15) == 0, "topk impl 2: item_emb must be 16-byte aligned");
-  const TcWorkspace w = tc_carve((char*)d->workspace, n_q, d->n_items, d->d);
+  const TcWorkspace w = tc_carve((char*)d->workspace, n_q, d->n_items, d->d, d->k);
   return d->d == 64 ? launch_tc<64>(d, w, st) : launch_tc<128>(d, w, st);
 }
 
 }  // namespace srb
 
 // byte offset of the int32 fallback counter inside the workspace (diagnostics: how many users the
-// exact kernel had to re-run); the same for every width
+// exact kernel had to re-run); the same for every width and list length
 extern "C" int64_t srb_topk_fallback_count_offset(int32_t n_q, int32_t n_items) {
   if (n_q <= 0 || n_items <= 0) return -1;
-  const srb::TcWorkspace w = srb::tc_carve((char*)256, n_q, n_items, 64);
+  const srb::TcWorkspace w = srb::tc_carve((char*)256, n_q, n_items, 64, 1);
   return (int64_t)((char*)w.fb_count - (char*)256);
 }
 
+// O(n_q * cap(k) + n_items): the candidate buffers of long lists grow with k, never with the catalogue
 extern "C" int64_t srb_topk_workspace_bytes(int32_t n_q, int32_t n_items, int32_t d, int32_t k) {
-  (void)k;
   if (n_q <= 0 || n_items <= 0 || d <= 0) return 0;
-  return srb::tc_carve(nullptr, n_q, n_items, d).bytes;
+  return srb::tc_carve(nullptr, n_q, n_items, d, k).bytes;
 }

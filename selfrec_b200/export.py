@@ -15,8 +15,10 @@ own [Ug, d] user block and rated rows (shard_rank.ShardRanker), and writes its o
 
 Users go through the ranker in chunks; each chunk's lists are copied to pinned host buffers on a side stream and from
 there into the memory-mapped part files, so the copy and file write of chunk k overlap the ranking of chunk k + 1 and
-host memory stays proportional to the chunk.  Lists longer than 32 come from dense [chunk, I] score rows (the 32-at-a-
-time path of ops.score_topk); their chunk is cut so those rows stay under WIDE_ROWS_BYTES.
+host memory stays proportional to the chunk.  Lists of 33..256 at d = 64 / 128 are ranked on the tensor cores like the
+short ones (ops.long_list_route): no score rows, only per-user candidate buffers, whose workspace cuts the chunk so it
+stays under LONG_WS_BYTES.  Other lists longer than 32 come from dense [chunk, I] score rows (the 32-at-a-time path of
+ops.score_topk); their chunk is cut so those rows stay under WIDE_ROWS_BYTES.
 
 Publishing is atomic, as for checkpoints: the part files go to a hidden sibling `.<name>.tmp`, are fsynced, and the
 directory is renamed into place in one os.replace (an older export of the same name is replaced only then).  Under a
@@ -37,6 +39,7 @@ FORMAT_VERSION = 1
 MANIFEST = "manifest.json"
 EXPORT_CHUNK = 1 << 16            # users per ranking call
 WIDE_ROWS_BYTES = 1 << 30         # cap on the dense [chunk, I] fp32 score rows of lists longer than 32
+LONG_WS_BYTES = 1 << 30           # cap on the ranking workspace of a chunk of long lists on the tensor cores
 
 
 def export_name(model_name, n):
@@ -99,7 +102,10 @@ class _Job:
             names = [data.id2user[int(u)] for u in uids]
             self._fn = lambda lo, hi: model._predict_topk(names[lo:hi], uids[lo:hi].astype(np.int32), n)
         if n > ops.TOPK_KERNEL_MAX and self.score_dtype == np.float32:
-            chunk = min(chunk, max(1, WIDE_ROWS_BYTES // (4 * I)))
+            if self.d is not None and ops.long_list_route(self.d, I, n):
+                chunk = long_list_chunk(chunk, I, self.d, n)
+            else:
+                chunk = min(chunk, max(1, WIDE_ROWS_BYTES // (4 * I)))
         self.uids, self.chunk = uids, chunk
         self.name = export_name(model.model_name, n)
         self.out_dir = out_dir
@@ -137,6 +143,16 @@ class _Job:
     def abort(self):
         if self.rank == 0:
             shutil.rmtree(self.tmp, ignore_errors=True)
+
+
+def long_list_chunk(chunk, n_items, d, n):
+    """The largest chunk <= `chunk` whose tensor-core ranking workspace of lists of n stays under LONG_WS_BYTES
+    (halving; at least 1)."""
+    from . import _lib
+    lib = _lib.load()
+    while chunk > 1 and lib.srb_topk_workspace_bytes(chunk, n_items, d, n) > LONG_WS_BYTES:
+        chunk //= 2
+    return chunk
 
 
 def _write_names(directory, fname, id2name, n):

@@ -508,7 +508,7 @@ def score_topk(user_emb, item_emb, users, rated_ptr, rated_idx, k, impl=0, stats
     d = user_emb.shape[1]
     if not 1 <= int(k) <= item_emb.shape[0]:
         raise SrbError(f"score_topk: k={k} must be in 1..n_items={item_emb.shape[0]} (find_k_largest seeds its heap with the first K candidates)")
-    if k > TOPK_KERNEL_MAX:
+    if k > TOPK_KERNEL_MAX and not (impl in (0, 2) and long_list_route(d, item_emb.shape[0], k, impl)):
         return _score_topk_wide(user_emb, item_emb, users, rated_ptr, rated_idx, int(k))
     out_ids = torch.empty((n_q, k), device=dev, dtype=torch.int32)
     out_sc = torch.empty((n_q, k), device=dev, dtype=torch.float32)
@@ -534,10 +534,20 @@ def score_topk(user_emb, item_emb, users, rated_ptr, rated_idx, k, impl=0, stats
 
 
 TOPK_KERNEL_MAX = 32  # list length of the selection kernels (one entry per lane)
+TOPK_TC_MAX = 256     # longest list of the tensor-core route (impl 2, d = 64 / 128)
+
+
+def long_list_route(d, n_items, k, impl=0):
+    """True when score_topk ranks a list of k > 32 on the tensor cores (impl 2, candidate buffers behind a running
+    threshold) rather than from dense score rows (_score_topk_wide): d in {64, 128}, k <= 256, and from 1024 items on
+    unless impl 2 is asked for explicitly."""
+    return (TOPK_KERNEL_MAX < int(k) <= TOPK_TC_MAX and int(d) in (64, 128)
+            and (int(impl) == 2 or (int(impl) == 0 and int(n_items) >= 1024)))
 
 
 def _score_topk_wide(user_emb, item_emb, users, rated_ptr, rated_idx, k):
-    """item.ranking.topN above 32 (e.g. 10,20,50): the selection kernels keep 32 entries per user, so the list is
+    """Lists above 32 off the tensor-core route (other widths, small catalogues, k > 256; long_list_route): the
+    selection kernels keep 32 entries per user, so the list is
     extracted 32 at a time from dense score rows -- srb_score_rows (the exact fp32 fma chains of predict()), the rated
     items masked with -10e8 like graph_recommender.py:48-50, srb_topk_rows, the winners struck out, repeat -- in
     user blocks of 2048.  Same selection rule (strictly greater replaces the minimum: earliest ids win ties at the
@@ -701,8 +711,9 @@ def adam_step(p, m, v, g, scalars, beta1=0.9, beta2=0.999, eps=1e-8):
 
 
 def rank_hit_masks(topk_ids, users, test_ptr, test_idx):
-    """uint64 mask per query row: bit r set iff topk_ids[q, r] is a test item of users[q] (k <= 64).
-    topk_ids: device int32 [n_q, k]; users / test_ptr / test_idx: int32 arrays or tensors."""
+    """Hit masks of the ranked lists: bit r set iff topk_ids[q, r] is a test item of users[q].  k <= 64: one
+    uint64 per query row, int64 [n_q]; 64 < k <= 256: ceil(k / 64) words per row, int64 [n_q, W], bit r % 64 of
+    word r // 64.  topk_ids: device int32 [n_q, k]; users / test_ptr / test_idx: int32 arrays or tensors."""
     lib = _lib.require_device()
     dev = topk_ids.device
     ids = topk_ids.contiguous()
@@ -712,7 +723,8 @@ def rank_hit_masks(topk_ids, users, test_ptr, test_idx):
     users, test_ptr, test_idx = to(users), to(test_ptr), to(test_idx)
     if test_idx.numel() == 0:
         test_idx = torch.zeros(1, dtype=torch.int32, device=dev)
-    out = torch.zeros(ids.shape[0], dtype=torch.int64, device=dev)
+    words = (ids.shape[1] + 63) // 64
+    out = torch.zeros((ids.shape[0],) if words == 1 else (ids.shape[0], words), dtype=torch.int64, device=dev)
     _lib.check(lib.srb_rank_hit_masks(_p(ids), ids.shape[0], ids.shape[1], _p(users), _p(test_ptr), _p(test_idx), _p(out), _stream()),
                "srb_rank_hit_masks")
     return out

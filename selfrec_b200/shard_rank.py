@@ -127,7 +127,8 @@ class ShardRanker:
         return ops.score_topk(user_block, item_emb, rows.astype(np.int32), *self.rated, k)
 
     def local_hit_masks(self, user_block, item_emb, uids, k):
-        """fast_evaluation's 64-bit hit masks (ops.rank_hit_masks, k <= 64) of the queried users this rank owns."""
+        """fast_evaluation's hit masks (ops.rank_hit_masks: int64 [n] for k <= 64, [n, ceil(k / 64)] up to 256) of the
+        queried users this rank owns."""
         import torch
         from . import ops
         if self._test is None:
@@ -136,7 +137,8 @@ class ShardRanker:
         _, rows = owned_positions(uids, self.rank, self.world)
         ids, _ = self.local_topk(user_block, item_emb, uids, k)
         if rows.size == 0:
-            return torch.empty(0, dtype=torch.int64, device=ids.device)
+            words = (k + 63) // 64
+            return torch.empty((0,) if words == 1 else (0, words), dtype=torch.int64, device=ids.device)
         return ops.rank_hit_masks(ids, rows.astype(np.int32), *self._test)
 
     def gather(self, local, uids):

@@ -40,10 +40,15 @@ def ranking_evaluation(origin, res, N):
 def ranking_evaluation_from_masks(n_test, masks, N):
     """Same strings as ranking_evaluation, from per-user hit masks (bit r of masks[q] = the item at rank r is
     a test item of that user; ops.rank_hit_masks) and n_test[q] = len(origin[user]), both in test-set order.
+    masks is one 64-bit word per user, or [n, W] words per user for lists longer than 64 (bit r % 64 of word
+    r // 64).
     Every float expression is the reference's (util/evaluation.py:9-15, 45-53, 85-97, 135-162) evaluated on
     the same operands in the same order, so the rounded values are identical."""
     n_test = [int(x) for x in n_test]
-    masks = [int(m) & 0xFFFFFFFFFFFFFFFF for m in masks]
+    if getattr(masks, "ndim", 1) == 2:
+        masks = [sum((int(w) & 0xFFFFFFFFFFFFFFFF) << (64 * j) for j, w in enumerate(row)) for row in masks]
+    else:
+        masks = [int(m) & 0xFFFFFFFFFFFFFFFF for m in masks]
     if len(n_test) != len(masks):
         print("The Lengths of test set and predicted set do not match!")
         exit(-1)
