@@ -5,20 +5,17 @@
 //   candidates[rated] = -10e8             graph_recommender.py:48-50
 //   find_k_largest(max_N, candidates)     util/algorithm.py:144-156
 //
-// One CTA scores 32 users against the whole catalogue in tiles of 128 items.  Each score is
-// an fp32 fma chain over k = 0..d-1 (exactly the oracle's loop, so scores are bit-identical).
-// The warp that computed a user's scores also owns that user's top-k list: one list entry
-// per lane, kept sorted by (score desc, id desc); a candidate enters iff score > current
-// k-th score (strict, like the reference's heapreplace test) and the last entry -- the
-// lexicographically smallest (score, id), i.e. what heapq would pop -- is evicted.  Items
-// are visited in id order, so the final SET equals find_k_largest's, ties included.
+// One CTA scores 32 users against the whole catalogue in tiles of 128 items, each score the
+// exact fp32 chain of rank_common.cuh.  The warp that computed a user's scores also owns that
+// user's top-k list (list_offer32, one entry per lane) and visits the items in id order, so the
+// final set equals find_k_largest's, ties included.
 #include "common.cuh"
+#include "rank_common.cuh"
 
 namespace srb {
 
 constexpr int TK_TM = 32;   // users per CTA
 constexpr int TK_TN = 128;  // items per tile
-constexpr float TK_MASKED = -1e9f;  // -10e8
 
 struct TopkArgs {
   const float* user_emb;
@@ -96,6 +93,7 @@ __global__ void __launch_bounds__(256) score_topk_kernel(const TopkArgs a) {
     for (int r = 0; r < 4; ++r)
 #pragma unroll
       for (int c = 0; c < 4; ++c) s[r][c] = 0.f;
+    // register-blocked 4 x 4 form of exact_score (rank_common.cuh): each s[r][c] is the same chain, k = 0..D-1 from +0
 #pragma unroll 8
     for (int k = 0; k < D; ++k) {
       const float4 uv = *reinterpret_cast<const float4*>(&Us[k][ty * 4]);
@@ -134,26 +132,7 @@ __global__ void __launch_bounds__(256) score_topk_kernel(const TopkArgs a) {
       }
       // sequential (id-ordered) insertion, 32 candidates per round
 #pragma unroll
-      for (int c = 0; c < 4; ++c) {
-        const float sc = s[r][c];
-        const int id = n0 + lane + 32 * c;
-        float thr = __shfl_sync(SRB_FULL_MASK, ls[r], K - 1);
-        unsigned m = __ballot_sync(SRB_FULL_MASK, sc > thr);
-        while (m) {
-          const int src = __ffs(m) - 1;
-          m &= m - 1;
-          const float cs = __shfl_sync(SRB_FULL_MASK, sc, src);
-          const int cid = __shfl_sync(SRB_FULL_MASK, id, src);
-          thr = __shfl_sync(SRB_FULL_MASK, ls[r], K - 1);
-          if (cs > thr) {
-            const int pos = __popc(__ballot_sync(SRB_FULL_MASK, lane < K && ls[r] > cs));
-            const float ps = __shfl_up_sync(SRB_FULL_MASK, ls[r], 1);
-            const int pi = __shfl_up_sync(SRB_FULL_MASK, li[r], 1);
-            if (lane > pos && lane < K) ls[r] = ps, li[r] = pi;
-            if (lane == pos) ls[r] = cs, li[r] = cid;
-          }
-        }
-      }
+      for (int c = 0; c < 4; ++c) list_offer32(ls[r], li[r], s[r][c], n0 + lane + 32 * c, K);
     }
   }
 #pragma unroll
@@ -167,67 +146,63 @@ __global__ void __launch_bounds__(256) score_topk_kernel(const TopkArgs a) {
   }
 }
 
-// top-k of precomputed score rows (models whose predict() is not a single dot product,
-// SURVEY 8b): one warp per row, same sequential insertion rule as above.
-__global__ void __launch_bounds__(256) topk_rows_kernel(const float* scores, int n_q, int n_items, int k, int32_t* out_ids,
-                                                        float* out_scores) {
+// top-k of score rows, one warp per row, same sequential insertion rule as above: precomputed rows of models whose
+// predict() is not a single dot product (SURVEY 8b), and the exact rows of impl 2's fast fallback.  Optional: n_q_dev,
+// a device-side row count (<= n_q); q_map, the output row of row q.
+__global__ void __launch_bounds__(256) topk_rows_kernel(const float* scores, int n_q, const int32_t* n_q_dev, const int32_t* q_map,
+                                                        int n_items, int k, int32_t* out_ids, float* out_scores) {
   const int lane = threadIdx.x & 31;
   const int q = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
-  if (q >= n_q) return;
+  if (q >= n_q || (n_q_dev && q >= *n_q_dev)) return;
   float ls = -INFINITY;
   int li = -1;
   const float* row = scores + (size_t)q * n_items;
   for (int n0 = 0; n0 < n_items; n0 += 32) {
     const int id = n0 + lane;
-    const float sc = (id < n_items) ? row[id] : -INFINITY;
-    float thr = __shfl_sync(SRB_FULL_MASK, ls, k - 1);
-    unsigned m = __ballot_sync(SRB_FULL_MASK, sc > thr);
-    while (m) {
-      const int src = __ffs(m) - 1;
-      m &= m - 1;
-      const float cs = __shfl_sync(SRB_FULL_MASK, sc, src);
-      const int cid = __shfl_sync(SRB_FULL_MASK, id, src);
-      thr = __shfl_sync(SRB_FULL_MASK, ls, k - 1);
-      if (cs > thr) {
-        const int pos = __popc(__ballot_sync(SRB_FULL_MASK, lane < k && ls > cs));
-        const float ps = __shfl_up_sync(SRB_FULL_MASK, ls, 1);
-        const int pi = __shfl_up_sync(SRB_FULL_MASK, li, 1);
-        if (lane > pos && lane < k) ls = ps, li = pi;
-        if (lane == pos) ls = cs, li = cid;
-      }
-    }
+    list_offer32(ls, li, (id < n_items) ? row[id] : -INFINITY, id, k);
   }
   if (lane < k) {
-    out_ids[(size_t)q * k + lane] = li;
-    out_scores[(size_t)q * k + lane] = ls;
+    const size_t orow = q_map ? (size_t)q_map[q] : (size_t)q;
+    out_ids[orow * k + lane] = li;
+    out_scores[orow * k + lane] = ls;
   }
 }
 
-// dense score rows out[q][i] = <user_emb[users[q]], item_emb[i]> (same fma chain as above):
-// the reference's predict() (XSimGCL.py:57-60) for callers that want the raw vector.
+// exact score of item i for user u, whose row `us` sits in shared memory; TK_MASKED when i is in u's sorted rated list
 template <int D>
-__global__ void __launch_bounds__(256) score_rows_kernel(const float* user_emb, const float* item_emb, const int32_t* users,
-                                                         int n_items, float* out) {
-  __shared__ float us[D];
-  const int q = blockIdx.y;
-  for (int k = threadIdx.x; k < D; k += blockDim.x) us[k] = user_emb[(size_t)users[q] * D + k];
-  __syncthreads();
-  const int i = blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= n_items) return;
+__device__ __forceinline__ float masked_score(const float* us, const float* item_emb, int i, int u, const int32_t* rated_ptr,
+                                              const int32_t* rated_idx) {
   const float* it = item_emb + (size_t)i * D;
-  float acc = 0.f;
-#pragma unroll 8
-  for (int k4 = 0; k4 < D / 4; ++k4) {
-    const float4 v = ldg4(it + k4 * 4);
-    acc = fmaf(us[k4 * 4 + 0], v.x, acc);
-    acc = fmaf(us[k4 * 4 + 1], v.y, acc);
-    acc = fmaf(us[k4 * 4 + 2], v.z, acc);
-    acc = fmaf(us[k4 * 4 + 3], v.w, acc);
+  const float acc = exact_score<D>([&](int c) { return reinterpret_cast<const float4*>(us)[c]; }, [&](int c) { return ldg4(it + c * 4); });
+  return (rated_ptr && sorted_contains(rated_idx, rated_ptr[u], rated_ptr[u + 1], i)) ? TK_MASKED : acc;
+}
+
+// dense score rows out[q][i] = <user_emb[users[q]], item_emb[i]>: the reference's predict() (XSimGCL.py:57-60) for
+// callers that want the raw vector, and, with the rated CSR and a device-side row count n_q_dev (<= n_q), the masked
+// rows of impl 2's fast fallback.  Rows stride over gridDim.y: the fallback usually has no rows, and a small grid.y
+// keeps that case cheap.
+template <int D>
+__global__ void __launch_bounds__(256) score_rows_kernel(const float* user_emb, const float* item_emb, const int32_t* users, int n_q,
+                                                         const int32_t* n_q_dev, const int32_t* rated_ptr, const int32_t* rated_idx,
+                                                         int n_items, float* out) {
+  __shared__ __align__(16) float us[D];
+  const int count = n_q_dev ? min(*n_q_dev, n_q) : n_q;
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  for (int q = blockIdx.y; q < count; q += gridDim.y) {
+    const int u = users[q];
+    __syncthreads();
+    for (int k = threadIdx.x; k < D; k += blockDim.x) us[k] = user_emb[(size_t)u * D + k];
+    __syncthreads();
+    if (i < n_items) out[(size_t)q * n_items + i] = masked_score<D>(us, item_emb, i, u, rated_ptr, rated_idx);
   }
-  out[(size_t)q * n_items + i] = acc;
 }
 
 int score_topk_tc(const srb_topk_desc* d, cudaStream_t st);  // score_topk_tc.cu
+
+static TopkArgs topk_args(const srb_topk_desc* d) {
+  return TopkArgs{d->user_emb, d->item_emb, d->n_items, d->users, d->n_q, d->rated_ptr, d->rated_idx, d->k, d->out_ids, d->out_scores,
+                  nullptr, nullptr, 0};
+}
 
 template <int D>
 static int launch_topk(const TopkArgs& a, cudaStream_t st) {
@@ -244,100 +219,20 @@ static int launch_topk(const TopkArgs& a, cudaStream_t st) {
 }
 
 // ---- fallback of impl 2: exact re-run of the users it could not certify (device-side list) ----
-// Fast path for the first `cap` of them: exact score rows spread over many CTAs + one warp per user
-// for the sequential top-k (a handful of users must not cost a full impl-1 pass over the catalogue).
-template <int D>
-__global__ void __launch_bounds__(256) fb_score_kernel(const float* __restrict__ user_emb, const float* __restrict__ item_emb,
-                                                      const int32_t* __restrict__ fb_users, const int32_t* __restrict__ fb_count,
-                                                      const int32_t* __restrict__ rated_ptr, const int32_t* __restrict__ rated_idx,
-                                                      int n_items, float* __restrict__ scratch, int cap) {
-  // the usual case is zero fallback users: a small grid.y that strides over the slots keeps that case cheap
-  const int count = min(*fb_count, cap);
-  __shared__ float us[D];
-  for (int slot = blockIdx.y; slot < count; slot += gridDim.y) {
-    const int u = fb_users[slot];
-    __syncthreads();
-    for (int k = threadIdx.x; k < D; k += blockDim.x) us[k] = user_emb[(size_t)u * D + k];
-    __syncthreads();
-    const int i = blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= n_items) continue;
-    const float* it = item_emb + (size_t)i * D;
-    float acc = 0.f;
-#pragma unroll 8
-    for (int k4 = 0; k4 < D / 4; ++k4) {
-      const float4 v = ldg4(it + k4 * 4);
-      acc = fmaf(us[k4 * 4 + 0], v.x, acc);
-      acc = fmaf(us[k4 * 4 + 1], v.y, acc);
-      acc = fmaf(us[k4 * 4 + 2], v.z, acc);
-      acc = fmaf(us[k4 * 4 + 3], v.w, acc);
-    }
-    if (rated_ptr) {  // binary search of item i in the user's sorted rated list
-      int lo = rated_ptr[u], hi = rated_ptr[u + 1];
-      while (lo < hi) {
-        const int mid = (lo + hi) >> 1;
-        const int v = rated_idx[mid];
-        if (v < i) lo = mid + 1; else hi = mid;
-      }
-      if (lo < rated_ptr[u + 1] && rated_idx[lo] == i) acc = TK_MASKED;
-    }
-    scratch[(size_t)slot * n_items + i] = acc;
-  }
-}
-
-__global__ void __launch_bounds__(256) fb_topk_kernel(const float* scratch, const int32_t* fb_rows, const int32_t* fb_count, int cap,
-                                                      int n_items, int k, int32_t* out_ids, float* out_scores) {
-  const int lane = threadIdx.x & 31;
-  const int slot = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
-  if (slot >= cap || slot >= *fb_count) return;
-  float ls = -INFINITY;
-  int li = -1;
-  const float* row = scratch + (size_t)slot * n_items;
-  for (int n0 = 0; n0 < n_items; n0 += 32) {
-    const int id = n0 + lane;
-    const float sc = (id < n_items) ? row[id] : -INFINITY;
-    float thr = __shfl_sync(SRB_FULL_MASK, ls, k - 1);
-    unsigned m = __ballot_sync(SRB_FULL_MASK, sc > thr);
-    while (m) {
-      const int src = __ffs(m) - 1;
-      m &= m - 1;
-      const float cs = __shfl_sync(SRB_FULL_MASK, sc, src);
-      const int cid = __shfl_sync(SRB_FULL_MASK, id, src);
-      thr = __shfl_sync(SRB_FULL_MASK, ls, k - 1);
-      if (cs > thr) {
-        const int pos = __popc(__ballot_sync(SRB_FULL_MASK, lane < k && ls > cs));
-        const float ps = __shfl_up_sync(SRB_FULL_MASK, ls, 1);
-        const int pi = __shfl_up_sync(SRB_FULL_MASK, li, 1);
-        if (lane > pos && lane < k) ls = ps, li = pi;
-        if (lane == pos) ls = cs, li = cid;
-      }
-    }
-  }
-  if (lane < k) {
-    const size_t orow = (size_t)fb_rows[slot];
-    out_ids[orow * k + lane] = li;
-    out_scores[orow * k + lane] = ls;
-  }
-}
-
 // Long lists (k > 32): one CTA per uncertified user at a time, at most `cap` users in flight (one scratch row each).
 // The CTA writes the user's exact masked row, finds the k-th largest score s* by a 4-pass 8-bit radix select, keeps
 // every score above it and, of the scores equal to it, find_k_largest's choice: among those within the first k items
 // (in id order) scoring >= s* -- the ones that entered the list -- the largest ids, as many as the list has room for
 // (tc_rescore_long_kernel states the rule), and writes the list score-descending, ties by id descending.
-__device__ __forceinline__ uint32_t fb_okey(float s) {  // order-preserving float -> uint32 (+0 and -0 alike)
-  const uint32_t b = __float_as_uint(s == 0.f ? 0.f : s);
-  return (b & 0x80000000u) ? ~b : (b | 0x80000000u);
-}
-
 template <int D>
 __global__ void __launch_bounds__(256, 1) fb_long_kernel(const float* __restrict__ user_emb, const float* __restrict__ item_emb,
                                                      const int32_t* __restrict__ fb_users, const int32_t* __restrict__ fb_rows,
                                                      const int32_t* __restrict__ fb_count, const int32_t* __restrict__ rated_ptr,
                                                      const int32_t* __restrict__ rated_idx, int n_items, int k, float* scratch,
                                                      int32_t* out_ids, float* out_scores) {
-  __shared__ float us[D];
+  __shared__ __align__(16) float us[D];
   __shared__ int hist[256];
-  __shared__ float sel_s[256];
+  __shared__ uint32_t sel_k[256];  // kept entries: okey of the score, id
   __shared__ int32_t sel_i[256];
   __shared__ int32_t tie_i[256];  // tied items that entered the list, in id order
   __shared__ int wsum[8];
@@ -351,27 +246,7 @@ __global__ void __launch_bounds__(256, 1) fb_long_kernel(const float* __restrict
     __syncthreads();
     for (int kk = tid; kk < D; kk += 256) us[kk] = user_emb[(size_t)u * D + kk];
     __syncthreads();
-    for (int i = tid; i < n_items; i += 256) {  // the fma chain and the mask of fb_score_kernel
-      const float* it = item_emb + (size_t)i * D;
-      float acc = 0.f;
-#pragma unroll 8
-      for (int k4 = 0; k4 < D / 4; ++k4) {
-        const float4 v = ldg4(it + k4 * 4);
-        acc = fmaf(us[k4 * 4 + 0], v.x, acc);
-        acc = fmaf(us[k4 * 4 + 1], v.y, acc);
-        acc = fmaf(us[k4 * 4 + 2], v.z, acc);
-        acc = fmaf(us[k4 * 4 + 3], v.w, acc);
-      }
-      if (rated_ptr) {
-        int lo = rated_ptr[u], hi = rated_ptr[u + 1];
-        while (lo < hi) {
-          const int mid = (lo + hi) >> 1;
-          if (rated_idx[mid] < i) lo = mid + 1; else hi = mid;
-        }
-        if (lo < rated_ptr[u + 1] && rated_idx[lo] == i) acc = TK_MASKED;
-      }
-      row[i] = acc;
-    }
+    for (int i = tid; i < n_items; i += 256) row[i] = masked_score<D>(us, item_emb, i, u, rated_ptr, rated_idx);
     __syncthreads();
     // radix select of the k-th largest key: pref = its key, need = how many of the entries equal to it to keep
     uint32_t pref = 0, pmask = 0;
@@ -380,7 +255,7 @@ __global__ void __launch_bounds__(256, 1) fb_long_kernel(const float* __restrict
       hist[tid] = 0;
       __syncthreads();
       for (int i = tid; i < n_items; i += 256) {
-        const uint32_t key = fb_okey(row[i]);
+        const uint32_t key = okey(row[i]);
         if ((key & pmask) == pref) atomicAdd(&hist[(key >> shift) & 255], 1);
       }
       __syncthreads();
@@ -398,10 +273,10 @@ __global__ void __launch_bounds__(256, 1) fb_long_kernel(const float* __restrict
     }
     // above the k-th: any slot of the first k - need; equal to it: the `need` smallest ids, visited in id order
     for (int i = tid; i < n_items; i += 256) {
-      const float sc = row[i];
-      if (fb_okey(sc) > pref) {
+      const uint32_t key = okey(row[i]);
+      if (key > pref) {
         const int p = atomicAdd(&s_nsel, 1);
-        sel_s[p] = sc;
+        sel_k[p] = key;
         sel_i[p] = i;
       }
     }
@@ -411,7 +286,7 @@ __global__ void __launch_bounds__(256, 1) fb_long_kernel(const float* __restrict
     __syncthreads();
     for (int base = 0; base < n_items && seen < k; base += 256) {
       const int i = base + tid;
-      const uint32_t key = i < n_items ? fb_okey(row[i]) : 0u;
+      const uint32_t key = i < n_items ? okey(row[i]) : 0u;
       const bool ge = i < n_items && key >= pref, tie = i < n_items && key == pref;
       const unsigned bg = __ballot_sync(SRB_FULL_MASK, ge), bt = __ballot_sync(SRB_FULL_MASK, tie);
       if (lane == 0) wsum[wid] = __popc(bg) | (__popc(bt) << 16);
@@ -438,24 +313,13 @@ __global__ void __launch_bounds__(256, 1) fb_long_kernel(const float* __restrict
     ties = s_ent;
     for (int t = tid; t < k; t += 256) {
       if (t >= k - need) {  // the largest `need` ids of the entered ties
-        const int i = tie_i[ties - (k - t)];
-        sel_s[t] = row[i];
-        sel_i[t] = i;
+        sel_k[t] = pref;
+        sel_i[t] = tie_i[ties - (k - t)];
       }
     }
     __syncthreads();
     const size_t orow = (size_t)fb_rows[slot];
-    for (int p = tid; p < k; p += 256) {
-      const uint32_t ek = fb_okey(sel_s[p]);
-      const int id = sel_i[p];
-      int pos = 0;
-      for (int j = 0; j < k; ++j) {
-        const uint32_t oj = fb_okey(sel_s[j]);
-        pos += (oj > ek) || (oj == ek && sel_i[j] > id);
-      }
-      out_ids[orow * k + pos] = id;
-      out_scores[orow * k + pos] = sel_s[p];
-    }
+    write_ranked(sel_k, sel_i, k, [](int) { return true; }, out_ids + orow * k, out_scores + orow * k);
   }
 }
 
@@ -467,26 +331,18 @@ static int score_topk_fallback_d(const srb_topk_desc* d, const int32_t* fb_users
                                               d->n_items, d->k, scratch, d->out_ids, d->out_scores);
     return post_launch("fb_long_kernel");
   }
-  // fast path: up to fb_cap users
+  // fast path for the first fb_cap users: exact score rows spread over many CTAs + one warp per user for the sequential
+  // top-k (a handful of users must not cost a full impl-1 pass over the catalogue)
   dim3 grid((d->n_items + 255) / 256, fb_cap < 8 ? fb_cap : 8);
-  fb_score_kernel<D><<<grid, 256, 0, st>>>(d->user_emb, d->item_emb, fb_users, fb_count, d->rated_ptr, d->rated_idx, d->n_items,
-                                            scratch, fb_cap);
-  SRB_TRY(post_launch("fb_score_kernel"));
-  fb_topk_kernel<<<(fb_cap + 7) / 8, 256, 0, st>>>(scratch, fb_rows, fb_count, fb_cap, d->n_items, d->k, d->out_ids, d->out_scores);
-  SRB_TRY(post_launch("fb_topk_kernel"));
+  score_rows_kernel<D><<<grid, 256, 0, st>>>(d->user_emb, d->item_emb, fb_users, fb_cap, fb_count, d->rated_ptr, d->rated_idx, d->n_items,
+                                             scratch);
+  SRB_TRY(post_launch("score_rows_kernel"));
+  topk_rows_kernel<<<(fb_cap + 7) / 8, 256, 0, st>>>(scratch, fb_cap, fb_count, fb_rows, d->n_items, d->k, d->out_ids, d->out_scores);
+  SRB_TRY(post_launch("topk_rows_kernel"));
   // slow path: everyone beyond fb_cap goes through the impl-1 kernel (CTAs without work exit at once)
   if (d->n_q <= fb_cap) return SRB_OK;
-  TopkArgs a;
-  a.user_emb = d->user_emb;
-  a.item_emb = d->item_emb;
-  a.n_items = d->n_items;
+  TopkArgs a = topk_args(d);
   a.users = fb_users;
-  a.n_q = d->n_q;
-  a.rated_ptr = d->rated_ptr;
-  a.rated_idx = d->rated_idx;
-  a.k = d->k;
-  a.out_ids = d->out_ids;
-  a.out_scores = d->out_scores;
   a.q_map = fb_rows;
   a.n_q_dev = fb_count;
   a.q_skip = fb_cap;
@@ -507,28 +363,14 @@ extern "C" int srb_score_topk(const srb_topk_desc* d, void* stream) {
   if (d->n_q == 0) return SRB_OK;  // empty query list: nothing to launch (pointers may be null)
   SRB_REQUIRE(d->user_emb && d->item_emb && d->users && d->out_ids && d->out_scores, "topk: null pointer");
   SRB_REQUIRE((d->rated_ptr == nullptr) == (d->rated_idx == nullptr), "topk: rated_ptr/rated_idx must both be set or both null");
-  SRB_REQUIRE(d->n_items >= 1 && d->n_q >= 0, "topk: bad shape");
+  SRB_REQUIRE(d->n_items >= 1, "topk: bad shape");
   SRB_REQUIRE(d->impl >= 0 && d->impl <= 2, "topk: bad impl");
-  if (d->n_q == 0) return SRB_OK;
   const bool tc = d->impl == 2 || (d->impl == 0 && (d->d == 64 || d->d == 128) && d->workspace != nullptr && d->n_items >= 1024);
   // impl 1 keeps one list entry per lane (k <= 32); impl 2 also takes the long lists (k <= 256)
   SRB_REQUIRE(d->k >= 1 && d->k <= (tc ? 256 : 32), "topk: k=%d unsupported (1..32; impl 2 at d = 64/128: 1..256)", d->k);
   SRB_REQUIRE(d->k <= 32 || d->k <= d->n_items, "topk: k=%d exceeds n_items=%d", d->k, d->n_items);
   if (tc) return srb::score_topk_tc(d, (cudaStream_t)stream);
-  srb::TopkArgs a;
-  a.user_emb = d->user_emb;
-  a.item_emb = d->item_emb;
-  a.n_items = d->n_items;
-  a.users = d->users;
-  a.n_q = d->n_q;
-  a.rated_ptr = d->rated_ptr;
-  a.rated_idx = d->rated_idx;
-  a.k = d->k;
-  a.out_ids = d->out_ids;
-  a.out_scores = d->out_scores;
-  a.q_map = nullptr;
-  a.n_q_dev = nullptr;
-  a.q_skip = 0;
+  const srb::TopkArgs a = srb::topk_args(d);
   switch (d->d) {
     case 16: return srb::launch_topk<16>(a, (cudaStream_t)stream);
     case 32: return srb::launch_topk<32>(a, (cudaStream_t)stream);
@@ -545,7 +387,7 @@ extern "C" int srb_topk_rows(const float* scores, int32_t n_q, int32_t n_items, 
   SRB_REQUIRE(k >= 1 && k <= 32, "topk_rows: k=%d unsupported (1..32)", k);
   SRB_REQUIRE(n_q >= 0 && n_items >= 1, "topk_rows: bad shape");
   if (n_q == 0) return SRB_OK;
-  srb::topk_rows_kernel<<<(n_q + 7) / 8, 256, 0, (cudaStream_t)stream>>>(scores, n_q, n_items, k, out_ids, out_scores);
+  srb::topk_rows_kernel<<<(n_q + 7) / 8, 256, 0, (cudaStream_t)stream>>>(scores, n_q, nullptr, nullptr, n_items, k, out_ids, out_scores);
   return srb::post_launch("topk_rows_kernel");
 }
 
@@ -557,11 +399,11 @@ extern "C" int srb_score_rows(const float* user_emb, const float* item_emb, int3
   dim3 grid((n_items + 255) / 256, n_q);
   cudaStream_t st = (cudaStream_t)stream;
   switch (d) {
-    case 16: srb::score_rows_kernel<16><<<grid, 256, 0, st>>>(user_emb, item_emb, users, n_items, out); break;
-    case 32: srb::score_rows_kernel<32><<<grid, 256, 0, st>>>(user_emb, item_emb, users, n_items, out); break;
-    case 64: srb::score_rows_kernel<64><<<grid, 256, 0, st>>>(user_emb, item_emb, users, n_items, out); break;
-    case 128: srb::score_rows_kernel<128><<<grid, 256, 0, st>>>(user_emb, item_emb, users, n_items, out); break;
-    case 256: srb::score_rows_kernel<256><<<grid, 256, 0, st>>>(user_emb, item_emb, users, n_items, out); break;
+    case 16: srb::score_rows_kernel<16><<<grid, 256, 0, st>>>(user_emb, item_emb, users, n_q, nullptr, nullptr, nullptr, n_items, out); break;
+    case 32: srb::score_rows_kernel<32><<<grid, 256, 0, st>>>(user_emb, item_emb, users, n_q, nullptr, nullptr, nullptr, n_items, out); break;
+    case 64: srb::score_rows_kernel<64><<<grid, 256, 0, st>>>(user_emb, item_emb, users, n_q, nullptr, nullptr, nullptr, n_items, out); break;
+    case 128: srb::score_rows_kernel<128><<<grid, 256, 0, st>>>(user_emb, item_emb, users, n_q, nullptr, nullptr, nullptr, n_items, out); break;
+    case 256: srb::score_rows_kernel<256><<<grid, 256, 0, st>>>(user_emb, item_emb, users, n_q, nullptr, nullptr, nullptr, n_items, out); break;
     default: srb::set_error("score_rows: unsupported d=%d (16, 32, 64, 128, 256)", d); return SRB_ERR_ARG;
   }
   return srb::post_launch("score_rows_kernel");
@@ -583,17 +425,7 @@ __global__ void __launch_bounds__(256) rank_hit_masks_kernel(const int32_t* __re
   unsigned long long mask = 0;
   for (int half = 0; half < 2; ++half) {
     const int r = wd * 64 + half * 32 + lane;
-    bool hit = false;
-    if (r < k) {
-      const int id = ids[(size_t)q * k + r];
-      int lo = beg, hi = end;
-      while (lo < hi) {
-        const int mid = (lo + hi) >> 1;
-        if (test_idx[mid] < id) lo = mid + 1;
-        else hi = mid;
-      }
-      hit = lo < end && test_idx[lo] == id;
-    }
+    const bool hit = r < k && sorted_contains(test_idx, beg, end, ids[(size_t)q * k + r]);
     mask |= (unsigned long long)__ballot_sync(SRB_FULL_MASK, hit) << (32 * half);
   }
   if (lane == 0) out[(size_t)q * words + wd] = mask;

@@ -29,6 +29,7 @@
 // memory behind a running threshold instead of the 24-slot list; tc_rescore_long_kernel (CTA per user) rescoring and
 // certifying them, fb_long_kernel (score_topk.cu) re-running the uncertified users (DESIGN 4.4).
 #include "common.cuh"
+#include "rank_common.cuh"
 #include "tc_common.cuh"
 
 namespace srb {
@@ -76,24 +77,46 @@ struct TcSmem {
   static constexpr uint32_t total = bar_off + 256;
 };
 
+// the workspace carved by tc_carve; the rescoring kernels read it and the caller's srb_topk_desc in place from the
+// parameter space (__grid_constant__)
+struct TcWorkspace {
+  float* ug;          // gathered user rows [n_q_pad][d]
+  float* unorm;       // ||u_q|| (tc_gather_kernel)
+  unsigned int* bmax; // bits of max ||item||: with unorm, the scale of the error bound E
+  float* cand_s;      // [n_q][2][24] approx scores
+  int32_t* cand_i;    // [n_q][2][24]
+  int32_t* cand_n;    // [n_q][2]
+  float* cand_thr;    // [n_q][2] min approx score of a full list, else -inf (long lists: final running threshold)
+  int32_t* fb_count;  // device counter of users needing the exact fallback
+  int32_t* fb_rows;   // their query rows
+  int32_t* fb_users;  // their user ids
+  float* fb_scratch;  // [fb_cap][n_items] exact score rows of the users re-run by the fast fallback
+  int32_t fb_cap;
+  float* buf_s;       // long lists: [n_q][2][cap] candidate buffers (empty at k <= 32)
+  int32_t* buf_i;
+  int32_t cap;
+  int64_t bytes;
+};
+
+// tc_score_kernel's arguments, taken from the desc and the workspace.  The kernel does not take those two whole as the
+// rescoring kernels do: ptxas then allocates its registers differently (102 -> 100 at d = 64, DESIGN 4.4), and the
+// hot kernel is kept as it was measured
 struct TcArgs {
-  const int32_t* users;      // original user ids per query row (for the rated CSR)
+  const int32_t* users;
   const int32_t* rated_ptr;
   const int32_t* rated_idx;
   int32_t n_q;
   int32_t n_items;
   int32_t ub;                // users per CTA (<= TC_UB)
-  float* cand_s;             // [n_q][2][24] approx scores
-  int32_t* cand_i;           // [n_q][2][24]
-  int32_t* cand_n;           // [n_q][2]
-  float* cand_thr;           // [n_q][2] min approx score of a full list, else -inf
-  // long lists (k > 32, tc_score_kernel<D, true>): per column half a candidate buffer of `cap` (score, id) slots
-  // behind a running threshold instead of the 24-slot list (DESIGN 4.4)
+  float* cand_s;
+  int32_t* cand_i;
+  int32_t* cand_n;
+  float* cand_thr;
   int32_t k;
   int32_t cap;
-  float* buf_s;              // [n_q][2][cap] approx scores
-  int32_t* buf_i;            // [n_q][2][cap]
-  const float* unorm;        // ||u_q|| and max ||item|| (tc_gather_kernel): the error bound E of the threshold
+  float* buf_s;
+  int32_t* buf_i;
+  const float* unorm;
   const unsigned int* bmax_bits;
 };
 
@@ -101,15 +124,6 @@ constexpr int TC_LONG_MAX = 256;  // longest list of the long-list route
 
 // per-half candidate capacity of a long list of k: room for the k best, the 2E band below them and a refill
 static int tc_long_cap(int k) { return (2 * k + 256 + 31) / 32 * 32; }
-
-// order-preserving map of a float to uint32 (+0 and -0 map alike) and back
-__device__ __forceinline__ uint32_t tc_okey(float s) {
-  const uint32_t b = __float_as_uint(s == 0.f ? 0.f : s);
-  return (b & 0x80000000u) ? ~b : (b | 0x80000000u);
-}
-__device__ __forceinline__ float tc_ofloat(uint32_t key) {
-  return __uint_as_float((key & 0x80000000u) ? (key & 0x7fffffffu) : ~key);
-}
 
 template <int D>
 struct TcVec;  // the D/32 floats of a row that one lane gathers
@@ -249,10 +263,10 @@ tc_score_kernel(const __grid_constant__ CUtensorMap tm_users, const __grid_const
     for (int b = 31; b >= 12; --b) {
       const uint32_t t = v | (1u << b);
       int c = 0;
-      for (int p = 0; p < a.cap; ++p) c += tc_okey(bs[p]) >= t;
+      for (int p = 0; p < a.cap; ++p) c += okey(bs[p]) >= t;
       if (c >= a.k) v = t;
     }
-    if (v != 0) thr = fmaxf(thr, tc_ofloat(v) - twoE);
+    if (v != 0) thr = fmaxf(thr, ofloat(v) - twoE);
     int kept = 0;
     for (int p = 0; p < a.cap; ++p) {
       const float s = bs[p];
@@ -401,37 +415,15 @@ tc_score_kernel(const __grid_constant__ CUtensorMap tm_users, const __grid_const
   }
 }
 
-struct RescoreArgs {
-  const float* ug;          // gathered user rows [n_q_pad][D]
-  const float* item_emb;
-  const float* unorm;
-  const unsigned int* bmax_bits;
-  const int32_t* users;
-  const int32_t* rated_ptr;
-  const float* cand_s;
-  const int32_t* cand_i;
-  const int32_t* cand_n;
-  const float* cand_thr;
-  int32_t n_q, n_items, k;
-  int32_t* out_ids;
-  float* out_scores;
-  int32_t* fb_count;        // device counter of users needing the exact fallback
-  int32_t* fb_rows;         // their query rows
-  int32_t* fb_users;        // their user ids
-  int32_t cap;              // long lists: per-half buffer capacity and the buffers of tc_score_kernel<D, true>
-  const float* buf_s;
-  const int32_t* buf_i;
-};
-
 template <int D>
-__global__ void __launch_bounds__(256) tc_rescore_kernel(const RescoreArgs a) {
+__global__ void __launch_bounds__(256) tc_rescore_kernel(const __grid_constant__ srb_topk_desc d, const __grid_constant__ TcWorkspace w) {
   const int lane = threadIdx.x & 31;
   const int q = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
-  if (q >= a.n_q) return;
-  const int cnt_a = a.cand_n[(size_t)q * 2], cnt_b = a.cand_n[(size_t)q * 2 + 1];
-  const int K = a.k;
-  const float bmax = __uint_as_float(*a.bmax_bits);
-  const float E = TcShape<D>::E * a.unorm[q] * bmax;  // TF32 truncation + k-step accumulation + slot tags
+  if (q >= d.n_q) return;
+  const int cnt_a = w.cand_n[(size_t)q * 2], cnt_b = w.cand_n[(size_t)q * 2 + 1];
+  const int K = d.k;
+  const float bmax = __uint_as_float(*w.bmax);
+  const float E = TcShape<D>::E * w.unorm[q] * bmax;  // TF32 truncation + k-step accumulation + slot tags
   // ---- prune by approximate score before any exact work ----
   // Every exact score lies within E of its approximate score.  Let a_K be the K-th largest approximate score of the
   // candidates: K candidates have an exact score >= a_K - E, so one whose approximate score is below a_K - 2E is beaten
@@ -448,8 +440,8 @@ __global__ void __launch_bounds__(256) tc_rescore_kernel(const RescoreArgs a) {
     for (int h = 0; h < 2; ++h) {
       const int c = lane + 32 * h;
       have[h] = c < TC_CAND && (c % TC_LIST) < ((c < TC_LIST) ? cnt_a : cnt_b);
-      ap[h] = have[h] ? a.cand_s[(size_t)q * TC_CAND + c] : -INFINITY;
-      cid[h] = have[h] ? a.cand_i[(size_t)q * TC_CAND + c] : 0x7fffffff;
+      ap[h] = have[h] ? w.cand_s[(size_t)q * TC_CAND + c] : -INFINITY;
+      cid[h] = have[h] ? w.cand_i[(size_t)q * TC_CAND + c] : 0x7fffffff;
     }
     float cut = -INFINITY;
     if (cnt_a + cnt_b > K) {
@@ -487,23 +479,13 @@ __global__ void __launch_bounds__(256) tc_rescore_kernel(const RescoreArgs a) {
     s[h] = -INFINITY;
     if (h == 1 && cnt <= 32) continue;  // warp-uniform
     if (mine[h]) id[h] = sv[c];
-    // exact score: the same fp32 fma chain over k = 0..D-1 as impl 1 and the oracle
     if (mine[h]) {
-      const float* u = a.ug + (size_t)q * D;
-      const float4* it = reinterpret_cast<const float4*>(a.item_emb + (size_t)id[h] * D);
-      float4 iv[D / 4];  // the whole row in flight at once: this kernel is bound by the latency of these gathers
+      const float4* u = reinterpret_cast<const float4*>(w.ug + (size_t)q * D);
+      const float4* it = reinterpret_cast<const float4*>(d.item_emb + (size_t)id[h] * D);
+      float4 iv[D / 4];  // the whole row in flight before the first fma: this kernel is bound by the latency of these gathers
 #pragma unroll
-      for (int k4 = 0; k4 < D / 4; ++k4) iv[k4] = __ldg(it + k4);
-      float acc = 0.f;
-#pragma unroll
-      for (int k4 = 0; k4 < D / 4; ++k4) {
-        const float4 uv = *reinterpret_cast<const float4*>(u + k4 * 4);
-        acc = fmaf(uv.x, iv[k4].x, acc);
-        acc = fmaf(uv.y, iv[k4].y, acc);
-        acc = fmaf(uv.z, iv[k4].z, acc);
-        acc = fmaf(uv.w, iv[k4].w, acc);
-      }
-      s[h] = acc;
+      for (int c = 0; c < D / 4; ++c) iv[c] = __ldg(it + c);
+      s[h] = exact_score<D, D / 4>([&](int c) { return u[c]; }, [&](int c) { return iv[c]; });
     }
   }
   // rank of my candidates by item id (ids are distinct; empty slots carry INT_MAX and never count)
@@ -531,35 +513,30 @@ __global__ void __launch_bounds__(256) tc_rescore_kernel(const RescoreArgs a) {
     const float2 e = mo[t];
     const float cs = e.x;
     if (cs > thr) {
-      const int cid = __float_as_int(e.y);
-      const int pos = __popc(__ballot_sync(SRB_FULL_MASK, lane < K && ls > cs));
-      const float ps = __shfl_up_sync(SRB_FULL_MASK, ls, 1);
-      const int pi = __shfl_up_sync(SRB_FULL_MASK, li, 1);
-      if (lane > pos && lane < K) ls = ps, li = pi;
-      if (lane == pos) ls = cs, li = cid;
+      list_insert(ls, li, cs, __float_as_int(e.y), K);
       thr = __shfl_sync(SRB_FULL_MASK, ls, K - 1);
     }
   }
   // exactness test
   const float kth = __shfl_sync(SRB_FULL_MASK, ls, K - 1);
-  const float thr32 = fmaxf(a.cand_thr[(size_t)q * 2], a.cand_thr[(size_t)q * 2 + 1]);
+  const float thr32 = fmaxf(w.cand_thr[(size_t)q * 2], w.cand_thr[(size_t)q * 2 + 1]);
   int deg = 0;
-  if (a.rated_ptr) {
-    const int u = a.users[q];
-    deg = a.rated_ptr[u + 1] - a.rated_ptr[u];
+  if (d.rated_ptr) {
+    const int u = d.users[q];
+    deg = d.rated_ptr[u + 1] - d.rated_ptr[u];
   }
-  const bool unsafe = (a.n_items - deg < K) || !(thr32 + E < kth);
+  const bool unsafe = (d.n_items - deg < K) || !(thr32 + E < kth);
   if (unsafe) {
     if (lane == 0) {
-      const int slot = atomicAdd(a.fb_count, 1);
-      a.fb_rows[slot] = q;
-      a.fb_users[slot] = a.users[q];
+      const int slot = atomicAdd(w.fb_count, 1);
+      w.fb_rows[slot] = q;
+      w.fb_users[slot] = d.users[q];
     }
     return;
   }
   if (lane < K) {
-    a.out_ids[(size_t)q * K + lane] = li;
-    a.out_scores[(size_t)q * K + lane] = ls;
+    d.out_ids[(size_t)q * K + lane] = li;
+    d.out_scores[(size_t)q * K + lane] = ls;
   }
 }
 
@@ -587,7 +564,7 @@ constexpr int TC_LONG_CAND = 2 * ((2 * TC_LONG_MAX + 256 + 31) / 32 * 32);  // b
 // thresholds), so the list is exact iff thr + E < the exact k-th score; otherwise, or when a buffer overflowed or
 // the user has fewer than k unrated items, the user goes to the exact fallback.
 template <int D>
-__global__ void __launch_bounds__(256) tc_rescore_long_kernel(const RescoreArgs a) {
+__global__ void __launch_bounds__(256) tc_rescore_long_kernel(const __grid_constant__ srb_topk_desc d, const __grid_constant__ TcWorkspace w) {
   __shared__ float s_ap[TC_LONG_CAND];       // approx scores, then the survivors' exact-score keys
   __shared__ int32_t s_id[TC_LONG_CAND];
   __shared__ int32_t s_sv[TC_LONG_CAND];     // survivor ids
@@ -598,21 +575,20 @@ __global__ void __launch_bounds__(256) tc_rescore_long_kernel(const RescoreArgs 
   __shared__ uint32_t s_kkey;
   const int q = blockIdx.x;
   const int tid = threadIdx.x;
-  const int K = a.k;
-  const int n0 = a.cand_n[(size_t)q * 2], n1 = a.cand_n[(size_t)q * 2 + 1];
+  const int K = d.k;
+  const int n0 = w.cand_n[(size_t)q * 2], n1 = w.cand_n[(size_t)q * 2 + 1];
   int deg = 0;
-  if (a.rated_ptr) {
-    const int u = a.users[q];
-    deg = a.rated_ptr[u + 1] - a.rated_ptr[u];
+  if (d.rated_ptr) {
+    const int u = d.users[q];
+    deg = d.rated_ptr[u + 1] - d.rated_ptr[u];
   }
-  const float E = TcShape<D>::E * a.unorm[q] * __uint_as_float(*a.bmax_bits);
-  bool unsafe = n0 < 0 || n1 < 0 || n0 + n1 < K || a.n_items - deg < K;
+  bool unsafe = n0 < 0 || n1 < 0 || n0 + n1 < K || d.n_items - deg < K;
   if (!unsafe) {
     const int n = n0 + n1;
     for (int c = tid; c < n; c += 256) {
-      const size_t o = (c < n0) ? (size_t)q * 2 * a.cap + c : ((size_t)q * 2 + 1) * a.cap + (c - n0);
-      s_ap[c] = a.buf_s[o];
-      s_id[c] = a.buf_i[o];
+      const size_t o = (c < n0) ? (size_t)q * 2 * w.cap + c : ((size_t)q * 2 + 1) * w.cap + (c - n0);
+      s_ap[c] = w.buf_s[o];
+      s_id[c] = w.buf_i[o];
     }
     if (tid == 0) s_cnt = 0;
     __syncthreads();
@@ -621,30 +597,20 @@ __global__ void __launch_bounds__(256) tc_rescore_long_kernel(const RescoreArgs 
     for (int b = 31; b >= 0; --b) {
       const uint32_t t = v | (1u << b);
       int c = 0;
-      for (int p = tid; p < n; p += 256) c += tc_okey(s_ap[p]) >= t;
+      for (int p = tid; p < n; p += 256) c += okey(s_ap[p]) >= t;
       if (tc_block_sum(c, red) >= K) v = t;
     }
-    const float cut = tc_ofloat(v) - 2.0f * E;
+    const float E = TcShape<D>::E * w.unorm[q] * __uint_as_float(*w.bmax);
+    const float cut = ofloat(v) - 2.0f * E;
     for (int p = tid; p < n; p += 256)
       if (s_ap[p] >= cut) s_sv[atomicAdd(&s_cnt, 1)] = s_id[p];
     __syncthreads();
     const int S = s_cnt;
-    // exact score: the same fp32 fma chain over k = 0..D-1 as impl 1 and the oracle
     uint32_t* s_ek = reinterpret_cast<uint32_t*>(s_ap);
-    const float* u = a.ug + (size_t)q * D;
+    const float4* u = reinterpret_cast<const float4*>(w.ug + (size_t)q * D);
     for (int p = tid; p < S; p += 256) {
-      const float4* it = reinterpret_cast<const float4*>(a.item_emb + (size_t)s_sv[p] * D);
-      float acc = 0.f;
-#pragma unroll 8
-      for (int k4 = 0; k4 < D / 4; ++k4) {
-        const float4 uv = *reinterpret_cast<const float4*>(u + k4 * 4);
-        const float4 iv = __ldg(it + k4);
-        acc = fmaf(uv.x, iv.x, acc);
-        acc = fmaf(uv.y, iv.y, acc);
-        acc = fmaf(uv.z, iv.z, acc);
-        acc = fmaf(uv.w, iv.w, acc);
-      }
-      s_ek[p] = tc_okey(acc);
+      const float4* it = reinterpret_cast<const float4*>(d.item_emb + (size_t)s_sv[p] * D);
+      s_ek[p] = okey(exact_score<D>([&](int c) { return u[c]; }, [&](int c) { return __ldg(it + c); }));
     }
     __syncthreads();
     for (int p = tid; p < S; p += 256) {
@@ -656,12 +622,12 @@ __global__ void __launch_bounds__(256) tc_rescore_long_kernel(const RescoreArgs 
         r += (oj > ek) || (oj == ek && s_sv[j] < id);
       }
       if (r == K - 1) {
-        s_kth = tc_ofloat(ek);
+        s_kth = ofloat(ek);
         s_kkey = ek;
       }
     }
     __syncthreads();
-    const float thr = fmaxf(a.cand_thr[(size_t)q * 2], a.cand_thr[(size_t)q * 2 + 1]);
+    const float thr = fmaxf(w.cand_thr[(size_t)q * 2], w.cand_thr[(size_t)q * 2 + 1]);
     unsafe = !(thr + E < s_kth);
     if (!unsafe) {
       const uint32_t kk = s_kkey;
@@ -693,48 +659,18 @@ __global__ void __launch_bounds__(256) tc_rescore_long_kernel(const RescoreArgs 
         keep[p] = k_;
       }
       __syncthreads();
-      for (int p = tid; p < S; p += 256) {
-        if (!keep[p]) continue;
-        const uint32_t ek = s_ek[p];
-        const int id = s_sv[p];
-        int pos = 0;
-        for (int j = 0; j < S; ++j) {
-          const uint32_t oj = s_ek[j];
-          pos += keep[j] && ((oj > ek) || (oj == ek && s_sv[j] > id));
-        }
-        a.out_ids[(size_t)q * K + pos] = id;
-        a.out_scores[(size_t)q * K + pos] = tc_ofloat(ek);
-      }
+      write_ranked(s_ek, s_sv, S, [&](int j) { return keep[j] != 0; }, d.out_ids + (size_t)q * K, d.out_scores + (size_t)q * K);
       return;
     }
   }
   if (tid == 0) {
-    const int slot = atomicAdd(a.fb_count, 1);
-    a.fb_rows[slot] = q;
-    a.fb_users[slot] = a.users[q];
+    const int slot = atomicAdd(w.fb_count, 1);
+    w.fb_rows[slot] = q;
+    w.fb_users[slot] = d.users[q];
   }
 }
 
 static int64_t tc_align(int64_t x) { return (x + 255) / 256 * 256; }
-
-struct TcWorkspace {
-  float* ug;
-  float* unorm;
-  unsigned int* bmax;
-  float* cand_s;
-  int32_t* cand_i;
-  int32_t* cand_n;
-  float* cand_thr;
-  int32_t* fb_count;
-  int32_t* fb_rows;
-  int32_t* fb_users;
-  float* fb_scratch;  // [fb_cap][n_items] exact score rows of the users re-run by the fast fallback
-  int32_t fb_cap;
-  float* buf_s;       // long lists: [n_q][2][cap] candidate buffers (empty at k <= 32)
-  int32_t* buf_i;
-  int32_t cap;
-  int64_t bytes;
-};
 
 static int tc_fb_cap(int n_items) {
   long long cap = (64ll << 20) / ((long long)n_items * 4);  // at most 64 MB of scratch
@@ -813,56 +749,15 @@ static int launch_tc(const srb_topk_desc* d, const TcWorkspace& w, cudaStream_t 
   SRB_REQUIRE(make_tmap_f32_rows(&tm_users, w.ug, (uint64_t)n_q_pad, D, TC_UB) == 0, "topk impl 2: cuTensorMapEncodeTiled(users) failed");
   SRB_REQUIRE(make_tmap_f32_rows(&tm_items, d->item_emb, (uint64_t)d->n_items, D, TC_TN) == 0,
               "topk impl 2: cuTensorMapEncodeTiled(items) failed");
-  TcArgs a;
-  a.users = d->users;
-  a.rated_ptr = d->rated_ptr;
-  a.rated_idx = d->rated_idx;
-  a.n_q = n_q;
-  a.n_items = d->n_items;
-  a.ub = ub;
-  a.cand_s = w.cand_s;
-  a.cand_i = w.cand_i;
-  a.cand_n = w.cand_n;
-  a.cand_thr = w.cand_thr;
-  a.k = d->k;
-  a.cap = w.cap;
-  a.buf_s = w.buf_s;
-  a.buf_i = w.buf_i;
-  a.unorm = w.unorm;
-  a.bmax_bits = w.bmax;
-  const bool lng = d->k > 32;
-  if (lng) {
+  const TcArgs a{d->users, d->rated_ptr, d->rated_idx, n_q, d->n_items, ub, w.cand_s, w.cand_i, w.cand_n, w.cand_thr, d->k, w.cap,
+                 w.buf_s, w.buf_i, w.unorm, w.bmax};
+  if (d->k > 32) {
     SRB_TRY((launch_tc_score<D, true>(tm_users, tm_items, a, blocks, st)));
-  } else {
-    SRB_TRY((launch_tc_score<D, false>(tm_users, tm_items, a, blocks, st)));
-  }
-  RescoreArgs r;
-  r.ug = w.ug;
-  r.item_emb = d->item_emb;
-  r.unorm = w.unorm;
-  r.bmax_bits = w.bmax;
-  r.users = d->users;
-  r.rated_ptr = d->rated_ptr;
-  r.cand_s = w.cand_s;
-  r.cand_i = w.cand_i;
-  r.cand_n = w.cand_n;
-  r.cand_thr = w.cand_thr;
-  r.n_q = n_q;
-  r.n_items = d->n_items;
-  r.k = d->k;
-  r.out_ids = d->out_ids;
-  r.out_scores = d->out_scores;
-  r.fb_count = w.fb_count;
-  r.fb_rows = w.fb_rows;
-  r.fb_users = w.fb_users;
-  r.cap = w.cap;
-  r.buf_s = w.buf_s;
-  r.buf_i = w.buf_i;
-  if (lng) {
-    tc_rescore_long_kernel<D><<<n_q, 256, 0, st>>>(r);
+    tc_rescore_long_kernel<D><<<n_q, 256, 0, st>>>(*d, w);
     SRB_TRY(post_launch("tc_rescore_long_kernel"));
   } else {
-    tc_rescore_kernel<D><<<(n_q + 7) / 8, 256, 0, st>>>(r);
+    SRB_TRY((launch_tc_score<D, false>(tm_users, tm_items, a, blocks, st)));
+    tc_rescore_kernel<D><<<(n_q + 7) / 8, 256, 0, st>>>(*d, w);
     SRB_TRY(post_launch("tc_rescore_kernel"));
   }
   return score_topk_fallback(d, w.fb_users, w.fb_rows, w.fb_count, w.fb_scratch, w.fb_cap, st);

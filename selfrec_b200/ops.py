@@ -519,7 +519,7 @@ def score_topk(user_emb, item_emb, users, rated_ptr, rated_idx, k, impl=0, stats
         rated_ptr, rated_idx = _i32(rated_ptr, dev), _i32(rated_idx, dev)
         desc.rated_ptr, desc.rated_idx = _p(rated_ptr), _p(rated_idx)
     if impl == 0:  # auto: tensor-core path for the embedding sizes it is written for, else the CUDA-core kernel
-        impl = 2 if (d in (64, 128) and item_emb.shape[0] >= 1024) else 1
+        impl = 2 if _tc_route(d, item_emb.shape[0], 0) else 1
     desc.k, desc.out_ids, desc.out_scores, desc.impl = k, _p(out_ids), _p(out_sc), impl
     ws = None
     if impl == 2:
@@ -541,8 +541,13 @@ def long_list_route(d, n_items, k, impl=0):
     """True when score_topk ranks a list of k > 32 on the tensor cores (impl 2, candidate buffers behind a running
     threshold) rather than from dense score rows (_score_topk_wide): d in {64, 128}, k <= 256, and from 1024 items on
     unless impl 2 is asked for explicitly."""
-    return (TOPK_KERNEL_MAX < int(k) <= TOPK_TC_MAX and int(d) in (64, 128)
-            and (int(impl) == 2 or (int(impl) == 0 and int(n_items) >= 1024)))
+    return TOPK_KERNEL_MAX < int(k) <= TOPK_TC_MAX and _tc_route(d, n_items, impl)
+
+
+def _tc_route(d, n_items, impl):
+    """True when impl 2 (tensor cores) ranks at this width: d in {64, 128}, and either asked for explicitly or, under
+    impl 0 (auto), from 1024 items on."""
+    return int(d) in (64, 128) and (int(impl) == 2 or (int(impl) == 0 and int(n_items) >= 1024))
 
 
 def _score_topk_wide(user_emb, item_emb, users, rated_ptr, rated_idx, k):
