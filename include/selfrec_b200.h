@@ -259,6 +259,15 @@ typedef struct srb_infonce_desc {
 int64_t srb_infonce_workspace_bytes(int32_t max_n, int32_t d, int32_t n_problems);
 int srb_infonce_fwd_bwd(const srb_infonce_desc* desc, void* stream);
 
+/* In-batch softmax loss, on the InfoNCE kernels and descriptor.
+ * Replaces batch_softmax_loss(user_emb, item_emb, temperature) util/loss_torch.py:25-32 as used by
+ *   SSL4Rec.py:33 (and imported by CL4SRec.py:7), plus its autograd backward:
+ *   loss_p = mean_i(-log(p_i + 1e-5)),  p_i = softmax(S)_ii,  S = normalize(v1) normalize(v2)^T / tau
+ * with v1 = user rows, v2 = item rows.  Same fields and workspace (srb_infonce_workspace_bytes) as
+ * srb_infonce_fwd_bwd; b_cos must be 1.  p_i comes from the row's log-sum-exp, so the loss stays
+ * finite where the reference's unshifted exp(S) overflows (1/tau > 88.7). */
+int srb_batch_softmax_fwd_bwd(const srb_infonce_desc* desc, void* stream);
+
 /* Standalone l2_reg_loss (util/loss_torch.py:18-22) on already-gathered embeddings, for the
  * op-level drop-in: loss = reg * sum_t ||x_t||_F / rows_t.  sumsq_dev: [4] device scratch kept
  * for the backward; gout_dev: device scalar upstream gradient. */

@@ -159,6 +159,7 @@ SYMBOLS = {
     "srb_bpr_l2_fwd_bwd": (C.c_int, [C.POINTER(BprDesc), VP]),
     "srb_infonce_workspace_bytes": (C.c_int64, [C.c_int32, C.c_int32, C.c_int32]),
     "srb_infonce_fwd_bwd": (C.c_int, [C.POINTER(InfoNceDesc), VP]),
+    "srb_batch_softmax_fwd_bwd": (C.c_int, [C.POINTER(InfoNceDesc), VP]),
     "srb_l2_reg_fwd": (C.c_int, [C.c_int32, C.POINTER(VP), c_i64p, c_i32p, C.c_float, VP, VP, VP]),
     "srb_l2_reg_bwd": (C.c_int, [C.c_int32, C.POINTER(VP), C.POINTER(VP), c_i64p, c_i32p, C.c_float, VP, VP, VP]),
     "srb_scatter_add_rows": (C.c_int, [VP, C.c_int32, VP, VP, C.c_int32, VP, C.c_int32, C.c_float, VP]),

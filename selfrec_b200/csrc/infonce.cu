@@ -14,6 +14,10 @@
 //                                                                            (6 n^2 d flop)
 //           (d = 256: nce_grad_wide_kernel, the column tile streamed in 128-wide halves)
 //   finish  back through F.normalize, loss = mean(lse - S_ii)
+//
+// The same kernels, with BSM = true (infonce_tc.cuh), replace batch_softmax_loss(user_emb, item_emb, temperature)
+// util/loss_torch.py:25-32 (SSL4Rec.py:33; CL4SRec imports it): only the per-row loss and a per-row gradient factor
+// differ.
 #include "common.cuh"
 #include "infonce_tc.cuh"
 
@@ -328,7 +332,17 @@ struct NceGradSmem {
   float red[8];
 };
 
-template <int D>
+// batch_softmax_loss: gscale times the row factor c_r of this thread's rows ty*4 + r (after sm.lse is written)
+__device__ __forceinline__ void bsm_row_scales(const NceProblem& p, const float* lse, int i0, int ty, int n, float gscale,
+                                               float (&gs)[4]) {
+#pragma unroll
+  for (int r = 0; r < 4; ++r) {
+    const int i = i0 + ty * 4 + r;
+    gs[r] = (i < n) ? gscale * bsm_row_coef(lse[ty * 4 + r], p.diag[i]) : 0.f;
+  }
+}
+
+template <int D, bool BSM>
 __global__ void __launch_bounds__(256) nce_grad_kernel(const NceArgs a) {
   pdl_wait();
   pdl_trigger();
@@ -355,14 +369,16 @@ __global__ void __launch_bounds__(256) nce_grad_kernel(const NceArgs a) {
     }
     const float lse = (i < n) ? M + logf(Lsum) : 0.f;
     sm.lse[threadIdx.x] = lse;
-    // loss contribution (split 0 only): sum_i (lse_i - S_ii)
-    float contrib = (split == 0 && i < n) ? lse - p.diag[i] : 0.f;
+    // loss contribution (split 0 only): sum_i loss_i
+    float contrib = (split == 0 && i < n) ? (BSM ? bsm_row_loss(lse, p.diag[i]) : lse - p.diag[i]) : 0.f;
     contrib = warp_sum(contrib);
     if ((threadIdx.x & 31) == 0) sm.red[threadIdx.x >> 5] = contrib;
   }
   __syncthreads();
   if (threadIdx.x == 0 && split == 0) atomicAdd(p.loss_acc, sm.red[0] + sm.red[1]);
   const float gscale = p.weight * a.inv_tau / (float)n;  // d loss / d S_ij = (P_ij - delta_ij) / n
+  float gs[4];  // BSM: gscale * c_r
+  if constexpr (BSM) bsm_row_scales(p, sm.lse, i0, ty, n, gscale, gs);
   float o1[4][CW];
 #pragma unroll
   for (int r = 0; r < 4; ++r)
@@ -389,7 +405,8 @@ __global__ void __launch_bounds__(256) nce_grad_kernel(const NceArgs a) {
         if (i < n && j < n) {
           g = exp2f((s[r][c] * a.inv_tau - lse) * L2E);
           if (i == j) g -= 1.f;
-          g *= gscale;
+          if constexpr (BSM) g *= gs[r];
+          else g *= gscale;
         }
         s[r][c] = g;
       }
@@ -469,6 +486,7 @@ struct NceGradWideSmem {
   float red[8];
 };
 
+template <bool BSM>
 __global__ void __launch_bounds__(256) nce_grad_wide_kernel(const NceArgs a) {
   pdl_wait();
   pdl_trigger();
@@ -496,13 +514,15 @@ __global__ void __launch_bounds__(256) nce_grad_wide_kernel(const NceArgs a) {
     }
     const float lse = (i < n) ? M + logf(Lsum) : 0.f;
     sm.lse[threadIdx.x] = lse;
-    float contrib = (split == 0 && i < n) ? lse - p.diag[i] : 0.f;
+    float contrib = (split == 0 && i < n) ? (BSM ? bsm_row_loss(lse, p.diag[i]) : lse - p.diag[i]) : 0.f;
     contrib = warp_sum(contrib);
     if ((threadIdx.x & 31) == 0) sm.red[threadIdx.x >> 5] = contrib;
   }
   __syncthreads();
   if (threadIdx.x == 0 && split == 0) atomicAdd(p.loss_acc, sm.red[0] + sm.red[1]);
   const float gscale = p.weight * a.inv_tau / (float)n;
+  float gs[4];  // BSM: gscale * c_r
+  if constexpr (BSM) bsm_row_scales(p, sm.lse, i0, ty, n, gscale, gs);
   float o1[2][4][CW];
 #pragma unroll
   for (int h = 0; h < 2; ++h)
@@ -555,7 +575,8 @@ __global__ void __launch_bounds__(256) nce_grad_wide_kernel(const NceArgs a) {
         if (i < n && j < n) {
           g = exp2f((s[r][c] * a.inv_tau - lse) * L2E);
           if (i == j) g -= 1.f;
-          g *= gscale;
+          if constexpr (BSM) g *= gs[r];
+          else g *= gscale;
         }
         s[r][c] = g;
       }
@@ -680,6 +701,8 @@ static int64_t nce_problem_floats(int np, int d) {
 // finish for the tensor-core path: pass A left dV1 unnormalised (sum_j exp(S_ij - 1/tau) v2_j) and the
 // denominators l_i in part_l; dV1hat = w/(n tau l_i) dV1, both sides get the diagonal term
 // (P_ii - 1) * w/(n tau) * vhat_other in exact fp32, then the same normalisation backward as nce_finish_kernel
+// (BSM: w/(n tau) times c_i)
+template <bool BSM>
 __global__ void __launch_bounds__(256) nce_tc_finish_kernel(const NceArgs a) {
   pdl_wait();
   pdl_trigger();
@@ -692,7 +715,8 @@ __global__ void __launch_bounds__(256) nce_tc_finish_kernel(const NceArgs a) {
   if (i >= n) return;
   const float li = p.part_l[i];
   const float pii = expf(p.diag[i] - a.inv_tau) / li;
-  const float gs = p.weight * a.inv_tau / (float)n;
+  float gs = p.weight * a.inv_tau / (float)n;
+  if constexpr (BSM) gs *= pii / (pii + BSM_EPS);
   const float cd = (pii - 1.f) * gs;
   const float2 v1 = *reinterpret_cast<const float2*>(p.V1 + (size_t)i * D + lane * 2);
   const float2 v2 = *reinterpret_cast<const float2*>(p.V2 + (size_t)i * D + lane * 2);
@@ -713,6 +737,7 @@ __global__ void __launch_bounds__(256) nce_tc_finish_kernel(const NceArgs a) {
 }
 
 // tensor-core pipeline: prep (exact rows + TF32 hi/lo parts) -> pass A (LSE + view-1 gradient) -> pass B -> finish
+template <bool BSM>
 static int nce_launch_tc(const NceArgs& a, int n_problems, cudaStream_t st) {
   const int np = a.np;
   const int d = NT_D;
@@ -771,17 +796,17 @@ static int nce_launch_tc(const NceArgs& a, int n_problems, cudaStream_t st) {
   const size_t smem = NtSmem::total + 1024;
   static bool attr_done = false;
   if (!attr_done) {
-    SRB_TRY(check_cuda(cudaFuncSetAttribute(nce_tc_kernel<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem), "nce tc attr"));
-    SRB_TRY(check_cuda(cudaFuncSetAttribute(nce_tc_kernel<2>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem), "nce tc attr"));
+    SRB_TRY(check_cuda(cudaFuncSetAttribute(nce_tc_kernel<1, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem), "nce tc attr"));
+    SRB_TRY(check_cuda(cudaFuncSetAttribute(nce_tc_kernel<2, BSM>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem), "nce tc attr"));
     attr_done = true;
   }
   dim3 grid(row_blocks, splits, n_problems);
-  SRB_TRY(launch_kernel(nce_tc_kernel<1>, grid, NT_THREADS, smem, st, "nce_tc_kernel<pass_a>", maps, t));
-  SRB_TRY(launch_kernel(nce_tc_kernel<2>, grid, NT_THREADS, smem, st, "nce_tc_kernel<pass_b>", maps, t));
-  return launch_kernel(nce_tc_finish_kernel, dim3((np + 7) / 8, n_problems), 256, 0, st, "nce_tc_finish_kernel", a);
+  SRB_TRY(launch_kernel(nce_tc_kernel<1, false>, grid, NT_THREADS, smem, st, "nce_tc_kernel<pass_a>", maps, t));
+  SRB_TRY(launch_kernel(nce_tc_kernel<2, BSM>, grid, NT_THREADS, smem, st, "nce_tc_kernel<pass_b>", maps, t));
+  return launch_kernel(nce_tc_finish_kernel<BSM>, dim3((np + 7) / 8, n_problems), 256, 0, st, "nce_tc_finish_kernel", a);
 }
 
-template <int D>
+template <int D, bool BSM>
 static int nce_launch(const NceArgs& a, int n_problems, cudaStream_t st) {
   const int np = a.np;
   {
@@ -792,10 +817,10 @@ static int nce_launch(const NceArgs& a, int n_problems, cudaStream_t st) {
     void (*grad)(const NceArgs);
     size_t grad_smem;
     if constexpr (D == NCE_WIDE_D) {
-      grad = nce_grad_wide_kernel;
+      grad = nce_grad_wide_kernel<BSM>;
       grad_smem = sizeof(NceGradWideSmem);
     } else {
-      grad = nce_grad_kernel<D>;
+      grad = nce_grad_kernel<D, BSM>;
       grad_smem = sizeof(NceGradSmem<D>);
     }
     static bool attr_done = false;
@@ -815,50 +840,47 @@ static int nce_launch(const NceArgs& a, int n_problems, cudaStream_t st) {
   return SRB_OK;
 }
 
-}  // namespace srb
-
-extern "C" int64_t srb_infonce_workspace_bytes(int32_t max_n, int32_t d, int32_t n_problems) {
-  if (max_n < 0 || d <= 0 || n_problems <= 0) return 0;
-  return srb::nce_problem_floats(srb::nce_np(max_n), d) * 4 * n_problems;
-}
-
-extern "C" int srb_infonce_fwd_bwd(const srb_infonce_desc* d, void* stream) {
-  SRB_REQUIRE(d != nullptr, "infonce: null desc");
-  SRB_REQUIRE(d->n_problems >= 1 && d->n_problems <= 4, "infonce: n_problems must be 1..4");
-  SRB_REQUIRE(d->temperature > 0.f, "infonce: temperature must be positive");
-  SRB_REQUIRE(d->d == 16 || d->d == 32 || d->d == 64 || d->d == 128 || d->d == 256, "infonce: unsupported d=%d (16, 32, 64, 128, 256)", d->d);
+// srb_infonce_fwd_bwd (BSM = false) and srb_batch_softmax_fwd_bwd (BSM = true): the same checks, workspace and routes
+template <bool BSM>
+static int nce_fwd_bwd(const srb_infonce_desc* d, void* stream) {
+  const char* what = BSM ? "batch_softmax" : "infonce";
+  SRB_REQUIRE(d != nullptr, "%s: null desc", what);
+  SRB_REQUIRE(d->n_problems >= 1 && d->n_problems <= 4, "%s: n_problems must be 1..4", what);
+  SRB_REQUIRE(d->temperature > 0.f, "%s: temperature must be positive", what);
+  SRB_REQUIRE(!BSM || d->b_cos, "%s: b_cos must be 1 (the loss normalises both inputs)", what);
+  SRB_REQUIRE(d->d == 16 || d->d == 32 || d->d == 64 || d->d == 128 || d->d == 256, "%s: unsupported d=%d (16, 32, 64, 128, 256)", what, d->d);
   int max_n = 0;
   for (int q = 0; q < d->n_problems; ++q) {
     const srb_infonce_problem& s = d->prob[q];
-    SRB_REQUIRE(s.table1 && s.table2 && s.idx && s.g1 && s.g2 && s.loss, "infonce: null pointer in problem %d", q);
-    SRB_REQUIRE(s.n >= 0, "infonce: negative n");
+    SRB_REQUIRE(s.table1 && s.table2 && s.idx && s.g1 && s.g2 && s.loss, "%s: null pointer in problem %d", what, q);
+    SRB_REQUIRE(s.n >= 0, "%s: negative n", what);
     if (s.n > max_n) max_n = s.n;
   }
   SRB_REQUIRE(d->workspace && d->workspace_bytes >= srb_infonce_workspace_bytes(max_n, d->d, d->n_problems),
-              "infonce: workspace too small (%lld < %lld)", (long long)d->workspace_bytes,
+              "%s: workspace too small (%lld < %lld)", what, (long long)d->workspace_bytes,
               (long long)srb_infonce_workspace_bytes(max_n, d->d, d->n_problems));
   if (max_n == 0) {
     for (int q = 0; q < d->n_problems; ++q)
-      SRB_TRY(srb::check_cuda(cudaMemsetAsync(d->prob[q].loss, 0, 4, (cudaStream_t)stream), "infonce memset"));
+      SRB_TRY(check_cuda(cudaMemsetAsync(d->prob[q].loss, 0, 4, (cudaStream_t)stream), what));
     return SRB_OK;
   }
-  srb::NceArgs a;
+  NceArgs a;
   a.n_problems = d->n_problems;
-  a.np = srb::nce_np(max_n);
+  a.np = nce_np(max_n);
   a.b_cos = d->b_cos;
   a.inv_tau = 1.0f / d->temperature;
   // enough CTAs for ~2 waves: row blocks x splits x problems
-  const int row_blocks = a.np / srb::NCE_T;
-  int splits = (2 * srb::sm_count() + row_blocks * d->n_problems - 1) / (row_blocks * d->n_problems);
+  const int row_blocks = a.np / NCE_T;
+  int splits = (2 * sm_count() + row_blocks * d->n_problems - 1) / (row_blocks * d->n_problems);
   if (splits < 1) splits = 1;
-  if (splits > srb::NCE_MAX_SPLITS) splits = srb::NCE_MAX_SPLITS;
+  if (splits > NCE_MAX_SPLITS) splits = NCE_MAX_SPLITS;
   if (splits > row_blocks) splits = row_blocks;
   a.splits = splits;
   float* w = reinterpret_cast<float*>(d->workspace);
-  const int64_t per = srb::nce_problem_floats(a.np, d->d);
+  const int64_t per = nce_problem_floats(a.np, d->d);
   for (int q = 0; q < d->n_problems; ++q) {
     const srb_infonce_problem& s = d->prob[q];
-    srb::NceProblem& p = a.p[q];
+    NceProblem& p = a.p[q];
     p.table1 = s.table1;
     p.table2 = s.table2;
     p.row_off1 = s.row_off1;
@@ -885,18 +907,29 @@ extern "C" int srb_infonce_fwd_bwd(const srb_infonce_desc* d, void* stream) {
     p.inv2 = t + a.np;
     p.diag = t + 2 * a.np;
     p.part_m = t + 3 * a.np;
-    p.part_l = t + 3 * a.np + (int64_t)srb::NCE_MAX_SPLITS * a.np;
-    p.lse = t + 3 * a.np + 2ll * srb::NCE_MAX_SPLITS * a.np;
+    p.part_l = t + 3 * a.np + (int64_t)NCE_MAX_SPLITS * a.np;
+    p.lse = t + 3 * a.np + 2ll * NCE_MAX_SPLITS * a.np;
     p.loss_acc = p.lse + a.np;
   }
   cudaStream_t st = (cudaStream_t)stream;
   // the tensor-core LSE pass shifts by the bound 1/tau of a cosine logit: needs exp(-2/tau) representable
-  if (d->d == 64 && d->b_cos && d->n_problems <= 2 && a.inv_tau <= 40.f) return srb::nce_launch_tc(a, d->n_problems, st);
+  if (d->d == 64 && d->b_cos && d->n_problems <= 2 && a.inv_tau <= 40.f) return nce_launch_tc<BSM>(a, d->n_problems, st);
   switch (d->d) {
-    case 16: return srb::nce_launch<16>(a, d->n_problems, st);
-    case 32: return srb::nce_launch<32>(a, d->n_problems, st);
-    case 64: return srb::nce_launch<64>(a, d->n_problems, st);
-    case 128: return srb::nce_launch<128>(a, d->n_problems, st);
-    default: return srb::nce_launch<256>(a, d->n_problems, st);
+    case 16: return nce_launch<16, BSM>(a, d->n_problems, st);
+    case 32: return nce_launch<32, BSM>(a, d->n_problems, st);
+    case 64: return nce_launch<64, BSM>(a, d->n_problems, st);
+    case 128: return nce_launch<128, BSM>(a, d->n_problems, st);
+    default: return nce_launch<256, BSM>(a, d->n_problems, st);
   }
 }
+
+}  // namespace srb
+
+extern "C" int64_t srb_infonce_workspace_bytes(int32_t max_n, int32_t d, int32_t n_problems) {
+  if (max_n < 0 || d <= 0 || n_problems <= 0) return 0;
+  return srb::nce_problem_floats(srb::nce_np(max_n), d) * 4 * n_problems;
+}
+
+extern "C" int srb_infonce_fwd_bwd(const srb_infonce_desc* d, void* stream) { return srb::nce_fwd_bwd<false>(d, stream); }
+
+extern "C" int srb_batch_softmax_fwd_bwd(const srb_infonce_desc* d, void* stream) { return srb::nce_fwd_bwd<true>(d, stream); }

@@ -9,6 +9,7 @@
 //   pass B  rows = view-2 rows j:  G' = exp(S^T - lse_i) * w/(n tau), i != j;  dV2 += G' V1   (needs every l_i)
 //   finish  scales dV1 by w/(n tau l_i), adds the diagonal term (P_ii - 1) w/(n tau) v_i in exact fp32, then the
 //           normalisation backward
+// batch_softmax_loss (BSM below) runs the same passes: its row factor c_i multiplies w/(n tau) in pass B and finish.
 // Each CTA owns a block of 128 rows and a strided subset of the 64-column tiles:
 //   warp 8        TMA producer: per tile, the column operand [64 x 64] (K-major over d, for S) and the same tile
 //                 from the transposed copy [64 d x 64 cols] (K-major over the column index, for G V), hi and lo
@@ -78,6 +79,21 @@ struct NtMaps {
   CUtensorMap v1r[2][2], v2r[2][2], v1c[2][2], v2c[2][2], v1t[2][2], v2t[2][2];
 };
 
+// The two losses over the in-batch softmax of S (row r: lse_r, p_r = exp(S_rr - lse_r)) differ only per row; BSM
+// selects batch_softmax_loss at compile time in the kernels of both paths:
+//   InfoNCE             loss_r = lse_r - S_rr          dL/dS_rj = (P_rj - delta_rj) / n
+//   batch_softmax_loss  loss_r = -log(p_r + 1e-5)      dL/dS_rj = c_r (P_rj - delta_rj) / n,  c_r = p_r / (p_r + 1e-5)
+// The reference (util/loss_torch.py:25-32) sums exp(S) without a shift and overflows once 1/tau > 88.7; here p_r comes
+// from the log-sum-exp and stays finite.
+constexpr float BSM_EPS = 1e-5f;  // the reference's 10e-6
+
+__device__ __forceinline__ float bsm_row_loss(float lse, float s_rr) { return -logf(expf(s_rr - lse) + BSM_EPS); }
+
+__device__ __forceinline__ float bsm_row_coef(float lse, float s_rr) {
+  const float p = expf(s_rr - lse);
+  return p / (p + BSM_EPS);
+}
+
 __device__ __forceinline__ int nt_n(const NtProblem& p) { return p.n_dev ? min(*p.n_dev, p.n) : p.n; }
 
 __device__ __forceinline__ float to_tf32_rna(float x) {
@@ -92,9 +108,11 @@ __device__ __forceinline__ float ex2_approx(float x) {  // 2^x, flush-to-zero, 2
   return y;
 }
 
-// mode 1: pass A (rows = view 1)   mode 2: pass B (rows = view 2)
-template <int MODE>
+// mode 1: pass A (rows = view 1)   mode 2: pass B (rows = view 2).  Pass A is the same for both losses: BSM (the
+// batch_softmax_loss row factor c_i, folded into pass B's column constants) applies to pass B only.
+template <int MODE, bool BSM>
 __global__ void __launch_bounds__(NT_THREADS, 1) nce_tc_kernel(const __grid_constant__ NtMaps maps, const NtArgs a) {
+  static_assert(MODE == 2 || !BSM, "pass A does not depend on the loss");
   pdl_wait();
   pdl_trigger();
   extern __shared__ __align__(1024) uint8_t nt_smem_raw[];
@@ -167,7 +185,8 @@ __global__ void __launch_bounds__(NT_THREADS, 1) nce_tc_kernel(const __grid_cons
     if (col < n) {
       const float lse = a.inv_tau + logf(P.lsum[col]);
       off = lg - lse * L2E;
-      contrib = lse - P.diag[col];
+      contrib = BSM ? bsm_row_loss(lse, P.diag[col]) : lse - P.diag[col];
+      if constexpr (BSM) off += log2f(bsm_row_coef(lse, P.diag[col]));  // c_col = 0 gives -inf: a zero column of G'
     }
     if (blockIdx.x == 0) {
       contrib = warp_sum(contrib);

@@ -430,8 +430,9 @@ def l2_reg_loss(reg, *args):
     return _L2Fn.apply(reg, *args)
 
 
-def infonce_raw(problems, d, temperature, b_cos=True, max_n=None, workspace=None):
-    """Run srb_infonce_fwd_bwd.  problems: list of dicts(table1, table2, idx, n, and optionally n_dev,
+def infonce_raw(problems, d, temperature, b_cos=True, max_n=None, workspace=None, batch_softmax=False):
+    """Run srb_infonce_fwd_bwd (srb_batch_softmax_fwd_bwd with batch_softmax=True, which needs b_cos).
+    problems: list of dicts(table1, table2, idx, n, and optionally n_dev,
     weight, row_off1, row_off2, scale1, scale2, and g1 / g2 output tensors to write into).
     workspace: optional uint8 device tensor to use instead of a fresh one (its whole size is offered).
     Returns (losses [P], [(g1, g2)])."""
@@ -466,7 +467,8 @@ def infonce_raw(problems, d, temperature, b_cos=True, max_n=None, workspace=None
         pr.loss = C.c_void_p(losses.data_ptr() + 4 * q)
         outs.append((g1, g2))
     desc.workspace, desc.workspace_bytes = _p(ws), ws_bytes
-    _lib.check(lib.srb_infonce_fwd_bwd(C.byref(desc), _stream()), "srb_infonce_fwd_bwd")
+    entry = "srb_batch_softmax_fwd_bwd" if batch_softmax else "srb_infonce_fwd_bwd"
+    _lib.check(getattr(lib, entry)(C.byref(desc), _stream()), entry)
     return losses, outs
 
 
@@ -492,6 +494,33 @@ class _InfoNceFn(torch.autograd.Function):
 
 def InfoNCE(view1, view2, temperature, b_cos=True):
     return _InfoNceFn.apply(view1, view2, float(temperature), bool(b_cos))
+
+
+class _BatchSoftmaxFn(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, user_emb, item_emb, temperature):
+        u, i = _f32c(user_emb, "batch_softmax_loss user_emb"), _f32c(item_emb, "batch_softmax_loss item_emb")
+        if u.dim() != 2 or u.shape != i.shape:
+            raise ValueError("batch_softmax_loss: user_emb and item_emb must both be [n, d]")
+        n, d = u.shape
+        if d not in _SUPPORTED_D:
+            raise SrbError(f"batch_softmax_loss: embedding size {d} unsupported (16, 32, 64, 128, 256)")
+        idx = torch.arange(n, device=u.device, dtype=torch.int32)
+        losses, outs = infonce_raw([dict(table1=u, table2=i, idx=idx, n=n, weight=1.0)], d, temperature, True,
+                                   batch_softmax=True)
+        ctx.save_for_backward(*outs[0])
+        return losses[0]
+
+    @staticmethod
+    def backward(ctx, go):
+        g1, g2 = ctx.saved_tensors
+        return g1 * go, g2 * go, None
+
+
+def batch_softmax_loss(user_emb, item_emb, temperature):
+    """util/loss_torch.py:25-32: mean_r -log(softmax(S)_rr + 1e-5), S = normalize(user) normalize(item)^T / temperature.
+    Computed in log-sum-exp form, so it stays finite below temperature 1/88.7, where the reference overflows."""
+    return _BatchSoftmaxFn.apply(user_emb, item_emb, float(temperature))
 
 
 # ----------------------------------------------------------------------------------------

@@ -256,3 +256,48 @@ def next_batch_pairwise(data, batch_size, n_negs=1):
         if b == 0:
             return
         yield u[:b].tolist(), i[:b].tolist(), j[: b * n_negs].tolist()
+
+
+def next_batch_sequence(data, batch_size, n_negs=1, max_len=50):
+    """util/sampler.py:84-112 (SASRec, BERT4Rec, CL4SRec): (seq, pos, y, neg, seq_len) int64 batches over a shuffled
+    copy of data.original_seq, with the same `random` draws as the reference.  Each row holds the last max_len - 1
+    items before the last one (seq) and the items after them (y); neg is one sample of as many catalogue ids
+    (1..item_num), drawn again until it shares no item with seq.  n_negs is accepted and unused, as in the reference.
+    Plain Python: shuffle and sample on the global `random` stream.  sample() picks positions, so drawing from
+    range(1, item_num + 1) takes the same draws as the reference's list of those ids."""
+    sequences = [s for _, s in data.original_seq]
+    random.shuffle(sequences)
+    catalogue = range(1, data.item_num + 1)
+    for ptr in range(0, len(sequences), batch_size):
+        rows = sequences[ptr:ptr + batch_size]
+        seq, pos, y, neg = (np.zeros((len(rows), max_len), dtype=np.int64) for _ in range(4))
+        seq_len = np.zeros(len(rows), dtype=np.int64)
+        for r, s in enumerate(rows):
+            start, end = (len(s) - max_len, max_len - 1) if len(s) > max_len else (0, len(s) - 1)
+            history = s[start:-1]
+            seq[r, :end] = history
+            pos[r, :end] = np.arange(1, end + 1)
+            y[r, :end] = s[start + 1:]
+            seen = set(history)
+            negatives = random.sample(catalogue, end)
+            while not seen.isdisjoint(negatives):
+                negatives = random.sample(catalogue, end)
+            neg[r, :end] = negatives
+            seq_len[r] = end
+        yield seq, pos, y, neg, seq_len
+
+
+def next_batch_sequence_for_test(data, batch_size, max_len=50):
+    """util/sampler.py:114-132 (base/seq_recommender.py test()): (seq, pos, seq_len) int64 batches of the last
+    max_len items of every sequence, in data.original_seq order.  Draws nothing from `random`."""
+    sequences = [s for _, s in data.original_seq]
+    for ptr in range(0, len(sequences), batch_size):
+        rows = sequences[ptr:ptr + batch_size]
+        seq, pos = (np.zeros((len(rows), max_len), dtype=np.int64) for _ in range(2))
+        seq_len = np.zeros(len(rows), dtype=np.int64)
+        for r, s in enumerate(rows):
+            end = min(len(s), max_len)
+            seq[r, :end] = s[len(s) - end:]
+            pos[r, :end] = np.arange(1, end + 1)
+            seq_len[r] = end
+        yield seq, pos, seq_len
