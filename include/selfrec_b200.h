@@ -323,8 +323,9 @@ int srb_adam_step(float* p, float* m, float* v, const float* g, int64_t n,
  *   out_ids  [n_q, k] int32, out_scores [n_q, k] fp32, score-descending
  * Selection follows find_k_largest's sequential semantics (strict > threshold, evict the
  * lexicographically smallest (score, id)); scores are exact fp32 fma chains over d.
- * k: 1..32 on impl 1; 1..256 on impl 2 (d = 64 or 128).  Longer lists, and lists over 32 at other
- * widths, are extracted 32 at a time from dense score rows (selfrec_b200/ops.py _score_topk_wide).
+ * k: 1..32 on impl 1; 1..256 on impl 2 (d = 16, 32, 64, 128 or 256).  Longer lists, and lists over 32
+ * that auto does not send to impl 2, are extracted 32 at a time from dense score rows
+ * (selfrec_b200/ops.py _score_topk_wide).
  * ------------------------------------------------------------------------------------- */
 typedef struct srb_topk_desc {
   const float* user_emb;
@@ -338,9 +339,10 @@ typedef struct srb_topk_desc {
   int32_t k;
   int32_t* out_ids;
   float* out_scores;
-  int32_t impl; /* 0 auto (impl 2 when d is 64 or 128, n_items >= 1024 and a workspace is given, else impl 1);
+  int32_t impl; /* 0 auto (impl 2 when n_items >= 1024, a workspace is given and either k <= 32 or d is 64 or
+                   128, else impl 1);
                    1 CUDA cores, exact fp32, k <= 32 (k > 32 is refused);
-                   2 (d = 64 or 128, k <= 256) wgmma TF32 candidates + exact fp32 rescoring + a per-user exactness
+                   2 (d = 16, 32, 64, 128 or 256, k <= 256) wgmma TF32 candidates + exact fp32 rescoring + a per-user exactness
                    certificate, uncertified users re-run by the exact path.  k <= 32: candidate lists of 2 x 24 per
                    user; 33 <= k <= 256: per-half candidate buffers behind a running threshold (DESIGN 4.4) */
   void* workspace; /* impl 2: srb_topk_workspace_bytes(n_q, n_items, d, k) bytes, 256-byte aligned;
@@ -350,8 +352,11 @@ typedef struct srb_topk_desc {
 
 int64_t srb_topk_workspace_bytes(int32_t n_q, int32_t n_items, int32_t d, int32_t k);
 /* byte offset (inside the impl-2 workspace) of the int32 count of users the exact fallback re-ran; the same at
-   d = 64 and d = 128 */
+   every d and k */
 int64_t srb_topk_fallback_count_offset(int32_t n_q, int32_t n_items);
+/* impl 2's error bound at width d: |approximate - exact score| <= E(d) * ||u|| * max_i ||item_i|| (DESIGN 4.4), the
+   constant of its certificate; -1 at a width impl 2 does not rank */
+float srb_topk_tc_error_bound(int32_t d);
 int srb_score_topk(const srb_topk_desc* desc, void* stream);
 /* Dense score rows out[q, i] = <user_emb[users[q]], item_emb[i]>, the reference's predict()
  * (XSimGCL.py:57-60); same fp32 fma chain as srb_score_topk. */

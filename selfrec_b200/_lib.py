@@ -180,6 +180,7 @@ SYMBOLS = {
     "srb_adam_step": (C.c_int, [VP, VP, VP, VP, C.c_int64, VP, C.c_double, C.c_double, C.c_float, VP]),
     "srb_topk_workspace_bytes": (C.c_int64, [C.c_int32, C.c_int32, C.c_int32, C.c_int32]),
     "srb_topk_fallback_count_offset": (C.c_int64, [C.c_int32, C.c_int32]),
+    "srb_topk_tc_error_bound": (C.c_float, [C.c_int32]),
     "srb_score_topk": (C.c_int, [C.POINTER(TopkDesc), VP]),
     "srb_score_rows": (C.c_int, [VP, VP, C.c_int32, VP, C.c_int32, C.c_int32, VP, VP]),
     "srb_topk_rows": (C.c_int, [VP, C.c_int32, C.c_int32, C.c_int32, VP, VP, VP]),

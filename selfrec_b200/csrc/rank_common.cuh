@@ -13,9 +13,9 @@ constexpr float TK_MASKED = -1e9f;  // -10e8, the score of a rated item (graph_r
 
 // The exact score of one (user, item) pair: acc = fma(u[k], i[k], acc) for k = 0..D-1 from acc = +0, so it is never
 // -0.  u4(c) / i4(c) return floats 4c..4c+3 of the user / item row; UNROLL sets how far their loads may run ahead.
+// A caller that walks the row in pieces passes the chain so far as acc (the next piece's floats indexed from 0).
 template <int D, int UNROLL = 8, class U4, class I4>
-__device__ __forceinline__ float exact_score(U4 u4, I4 i4) {
-  float acc = 0.f;
+__device__ __forceinline__ float exact_score(U4 u4, I4 i4, float acc = 0.f) {
 #pragma unroll UNROLL
   for (int c = 0; c < D / 4; ++c) {
     const float4 u = u4(c), i = i4(c);

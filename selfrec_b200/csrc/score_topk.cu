@@ -351,8 +351,13 @@ static int score_topk_fallback_d(const srb_topk_desc* d, const int32_t* fb_users
 
 int score_topk_fallback(const srb_topk_desc* d, const int32_t* fb_users, const int32_t* fb_rows, const int32_t* fb_count,
                         float* scratch, int fb_cap, cudaStream_t st) {
-  if (d->d == 128) return score_topk_fallback_d<128>(d, fb_users, fb_rows, fb_count, scratch, fb_cap, st);
-  return score_topk_fallback_d<64>(d, fb_users, fb_rows, fb_count, scratch, fb_cap, st);
+  switch (d->d) {  // the widths score_topk_tc accepts
+    case 16: return score_topk_fallback_d<16>(d, fb_users, fb_rows, fb_count, scratch, fb_cap, st);
+    case 32: return score_topk_fallback_d<32>(d, fb_users, fb_rows, fb_count, scratch, fb_cap, st);
+    case 128: return score_topk_fallback_d<128>(d, fb_users, fb_rows, fb_count, scratch, fb_cap, st);
+    case 256: return score_topk_fallback_d<256>(d, fb_users, fb_rows, fb_count, scratch, fb_cap, st);
+    default: return score_topk_fallback_d<64>(d, fb_users, fb_rows, fb_count, scratch, fb_cap, st);
+  }
 }
 
 }  // namespace srb
@@ -365,9 +370,11 @@ extern "C" int srb_score_topk(const srb_topk_desc* d, void* stream) {
   SRB_REQUIRE((d->rated_ptr == nullptr) == (d->rated_idx == nullptr), "topk: rated_ptr/rated_idx must both be set or both null");
   SRB_REQUIRE(d->n_items >= 1, "topk: bad shape");
   SRB_REQUIRE(d->impl >= 0 && d->impl <= 2, "topk: bad impl");
-  const bool tc = d->impl == 2 || (d->impl == 0 && (d->d == 64 || d->d == 128) && d->workspace != nullptr && d->n_items >= 1024);
+  // auto (impl 0): impl 2 from 1024 items on, at every width for lists of up to 32 and at d = 64 / 128 for longer ones
+  const bool tc_width = d->d == 64 || d->d == 128 || (d->k <= 32 && (d->d == 16 || d->d == 32 || d->d == 256));
+  const bool tc = d->impl == 2 || (d->impl == 0 && tc_width && d->workspace != nullptr && d->n_items >= 1024);
   // impl 1 keeps one list entry per lane (k <= 32); impl 2 also takes the long lists (k <= 256)
-  SRB_REQUIRE(d->k >= 1 && d->k <= (tc ? 256 : 32), "topk: k=%d unsupported (1..32; impl 2 at d = 64/128: 1..256)", d->k);
+  SRB_REQUIRE(d->k >= 1 && d->k <= (tc ? 256 : 32), "topk: k=%d unsupported (1..32; impl 2: 1..256)", d->k);
   SRB_REQUIRE(d->k <= 32 || d->k <= d->n_items, "topk: k=%d exceeds n_items=%d", d->k, d->n_items);
   if (tc) return srb::score_topk_tc(d, (cudaStream_t)stream);
   const srb::TopkArgs a = srb::topk_args(d);

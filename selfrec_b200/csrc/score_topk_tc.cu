@@ -4,15 +4,17 @@
 // Replaces GraphRecommender.test() base/graph_recommender.py:38-58 (predict XSimGCL.py:57-60,
 // mask :48-50, find_k_largest util/algorithm.py:144-156), same contract as impl 1.
 //
-// Both kernels are templated on the embedding size D in {64, 128}.
+// The kernels are templated on the embedding size D in {16, 32, 64, 128, 256}.
 //
 // Stage 1  tc_gather_kernel     users[q] rows -> contiguous [n_q, d] table (TMA cannot gather),
 //                               ||u_q||, max_i ||item_i||
 // Stage 2  tc_score_kernel      one CTA per block of UB <= 128 users, streaming the whole catalogue in
 //                               tiles of 128 items:
-//            warp 8     TMA producer: item tiles [128 x D] fp32 in 32-float k-chunks, 128B-swizzled, through a
-//                       2-stage mbarrier ring (D = 64: a stage is a whole tile; D = 128: a stage is one k-chunk,
-//                       four stages per tile, so the 64 KB user tile fits beside the ring -- DESIGN 4.4)
+//            warp 8     TMA producer: item tiles [128 x D] fp32 in 32-float k-chunks, 128B-swizzled, through an
+//                       mbarrier ring (D = 64: a stage is a whole tile; D = 128: a stage is one k-chunk, four stages
+//                       per tile, so the 64 KB user tile fits beside the ring; D = 16: a chunk is the 16 columns and
+//                       TMA's zero fill; D = 256: a stage is one item k-chunk and the users' same k-chunk, three
+//                       stages, since a resident 128 KB user tile would not fit -- DESIGN 4.4)
 //            warpgroups 0, 1  (64 users each): wgmma m64n128k8 kind tf32, D/8 k-steps per tile, accumulators in
 //                       registers -> staged to shared memory row-major -> select: thread = one user row x one
 //                       64-column half of the tile, rated-item cursor, per-thread top-24 candidate list
@@ -38,39 +40,44 @@ using namespace tc;
 
 constexpr int TC_TN = 128;        // items per tile (wgmma N)
 constexpr int TC_UB = 128;        // users per CTA: two consumer warpgroups of 64 (wgmma M)
-constexpr int TC_STAGES = 2;      // smem ring depth (a tile's select takes microseconds: one tile of prefetch is enough)
+constexpr int TC_STAGES = 2;      // smem ring depth at d <= 128 (a tile's select takes microseconds: one tile of prefetch is enough)
 constexpr int TC_LIST = 24;       // candidates per list; every user has two lists, one per column half of the tiles
 constexpr int TC_CAND = 2 * TC_LIST;
 constexpr int TC_THREADS = 256 + 32;   // warpgroups 0-1 MMA + select, warp 8 TMA
 constexpr int TC_SROW = TC_TN + 4;     // staged accumulator row stride (floats): conflict-free float4 row reads
 constexpr uint32_t TC_CHUNK_BYTES = 128 * 32 * 4;     // 16 KB: one k-chunk [128 rows][32] fp32 of a user or item tile
 
-// per-width layout: a tile row is D/32 k-chunks; a ring stage holds SC of them
+// per-width layout: a tile row is KC 32-float k-chunks (D = 16: one, half of it TMA's zero fill beyond the row, of which
+// the MMA reads the first 16 columns); a ring stage holds SC item chunks and, when the users stream (US), the users'
+// same chunk
 template <int D>
 struct TcShape {
-  static_assert(D == 64 || D == 128, "tensor-core ranking: D in {64, 128}");
-  static constexpr int KC = D / 32;                      // k-chunks per tile row
-  static constexpr int SC = (D == 64) ? 2 : 1;           // k-chunks per ring stage
-  static constexpr int SPT = KC / SC;                    // ring stages per item tile
-  static constexpr uint32_t STAGE_BYTES = SC * TC_CHUNK_BYTES;  // 32 KB (D = 64) / 16 KB (D = 128)
-  static constexpr uint32_t USER_BYTES = KC * TC_CHUNK_BYTES;   // 32 KB / 64 KB
+  static_assert(D == 16 || D == 32 || D == 64 || D == 128 || D == 256, "tensor-core ranking: D in {16, 32, 64, 128, 256}");
+  static constexpr int KC = D < 32 ? 1 : D / 32;          // k-chunks per tile row
+  static constexpr int KS = D < 32 ? D / 8 : 4;           // wgmma k-steps per k-chunk
+  static constexpr int SC = (D == 64) ? 2 : 1;            // item k-chunks per ring stage
+  static constexpr int SPT = KC / SC;                     // ring stages per item tile
+  static constexpr bool US = D == 256;                    // user chunks stream through the ring beside the items'
+  static constexpr int STAGES = US ? 3 : TC_STAGES;
+  static constexpr uint32_t STAGE_BYTES = (SC + US) * TC_CHUNK_BYTES;      // 32 KB (D = 64, 256) / 16 KB (others)
+  static constexpr uint32_t USER_BYTES = US ? 0 : KC * TC_CHUNK_BYTES;     // resident user tile: 16 / 16 / 32 / 64 KB
   // |approx - exact| <= E * ||u|| * max||i||: the TF32 operand term 2^-9 (independent of D), the accumulation term
-  // 2^-16 per 8 k-steps (it grows with the chain of k-steps: 2^-16 at D = 64, 2^-15 at D = 128) and 2^-18 for the
-  // slot tags and the final roundings (DESIGN 4.4)
-  static constexpr float E = 1.0f / 512.0f + (float)(D / 64) * (1.0f / 65536.0f) + 1.0f / 262144.0f;
+  // 2^-19 per k-step of 8 (it grows with the chain of D / 8 k-steps: 2^-18 at D = 16 ... 2^-14 at D = 256) and 2^-18
+  // for the slot tags and the final roundings (DESIGN 4.4)
+  static constexpr float E = 1.0f / 512.0f + (float)(D / 8) * (1.0f / 524288.0f) + 1.0f / 262144.0f;
 };
 
 template <int D>
 struct TcSmem {
   // dynamic shared memory, 1024-byte aligned base:
-  //   [0, U)            user tile    chunk c at c * 16 KB (warpgroup w's 64 rows at + w * 8 KB); U = 32 KB / 64 KB
-  //   [U, U + 2 S)      item stages  stage s, chunk c at U + s*S + c*16K; S = 32 KB (D = 64) / 16 KB (D = 128)
+  //   [0, U)            resident user tile: chunk c at c * 16 KB (warpgroup w's 64 rows at + w * 8 KB); U = 0 at D = 256
+  //   [U, U + N S)      N ring stages of S bytes: item chunk c at + c * 16 KB, then (D = 256) the users' chunk
   //   then the staged accumulators [2 warpgroups][64][TC_SROW] f32                  (66 KB)
   //   then candidate lists: scores [24][256] f32, ids [24][256] i32               (48 KB)
-  //   then barriers                                          total 210 KB + 256 B at both widths
+  //   then barriers         total 162 KB (D = 16, 32) / 210 KB (D = 64, 128, 256) + 256 B
   static constexpr uint32_t users_off = 0;
   static constexpr uint32_t items_off = TcShape<D>::USER_BYTES;
-  static constexpr uint32_t stage_off = items_off + TC_STAGES * TcShape<D>::STAGE_BYTES;
+  static constexpr uint32_t stage_off = items_off + TcShape<D>::STAGES * TcShape<D>::STAGE_BYTES;
   static constexpr uint32_t cand_s_off = stage_off + TC_UB * TC_SROW * 4;
   static constexpr uint32_t cand_i_off = cand_s_off + TC_LIST * 2 * TC_UB * 4;
   static constexpr uint32_t bar_off = cand_i_off + TC_LIST * 2 * TC_UB * 4;
@@ -126,7 +133,15 @@ constexpr int TC_LONG_MAX = 256;  // longest list of the long-list route
 static int tc_long_cap(int k) { return (2 * k + 256 + 31) / 32 * 32; }
 
 template <int D>
-struct TcVec;  // the D/32 floats of a row that one lane gathers
+struct TcVec;  // the D/32 floats of a row that one lane gathers (D = 16: lanes 0-15 one float each)
+template <>
+struct TcVec<16> {
+  using T = float;
+  static __device__ __forceinline__ T zero() { return 0.f; }
+  static __device__ __forceinline__ float ss(T v) { return v * v; }
+};
+template <>
+struct TcVec<32> : TcVec<16> {};
 template <>
 struct TcVec<64> {
   using T = float2;
@@ -139,6 +154,15 @@ struct TcVec<128> {
   static __device__ __forceinline__ T zero() { return make_float4(0.f, 0.f, 0.f, 0.f); }
   static __device__ __forceinline__ float ss(T v) { return v.x * v.x + v.y * v.y + v.z * v.z + v.w * v.w; }
 };
+struct alignas(16) TcF8 {
+  float4 a, b;
+};
+template <>
+struct TcVec<256> {
+  using T = TcF8;
+  static __device__ __forceinline__ T zero() { return TcF8{TcVec<128>::zero(), TcVec<128>::zero()}; }
+  static __device__ __forceinline__ float ss(T v) { return TcVec<128>::ss(v.a) + TcVec<128>::ss(v.b); }
+};
 
 template <int D>
 __global__ void __launch_bounds__(256) tc_gather_kernel(const float* __restrict__ user_emb, const int32_t* __restrict__ users, int n_q,
@@ -148,16 +172,18 @@ __global__ void __launch_bounds__(256) tc_gather_kernel(const float* __restrict_
   const int w = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
   // rows [0, n_q_pad): gathered user rows; rows [n_q_pad, n_q_pad + n_items): item norms
   using V = TcVec<D>;
-  constexpr int PL = D / 32;  // floats per lane
+  constexpr int PL = D < 32 ? 1 : D / 32;  // floats per lane
+  const bool ln = D >= 32 || lane < D;    // this lane holds floats of the row
   if (w < n_q_pad) {
     typename V::T v = V::zero();
-    if (w < n_q) v = *reinterpret_cast<const typename V::T*>(user_emb + (size_t)users[w] * D + lane * PL);
-    *reinterpret_cast<typename V::T*>(ug + (size_t)w * D + lane * PL) = v;
+    if (w < n_q && ln) v = *reinterpret_cast<const typename V::T*>(user_emb + (size_t)users[w] * D + lane * PL);
+    if (ln) *reinterpret_cast<typename V::T*>(ug + (size_t)w * D + lane * PL) = v;
     const float ss = warp_sum(V::ss(v));
     if (lane == 0 && w < n_q) unorm[w] = sqrtf(ss);
   } else if (w < n_q_pad + n_items) {
     const int i = w - n_q_pad;
-    const typename V::T v = *reinterpret_cast<const typename V::T*>(item_emb + (size_t)i * D + lane * PL);
+    typename V::T v = V::zero();
+    if (ln) v = *reinterpret_cast<const typename V::T*>(item_emb + (size_t)i * D + lane * PL);
     const float ss = warp_sum(V::ss(v));
     // non-negative floats order like uints; 38 k atomics on one word serialise, so look before touching it
     const unsigned int bits = __float_as_uint(sqrtf(ss));
@@ -174,15 +200,15 @@ tc_score_kernel(const __grid_constant__ CUtensorMap tm_users, const __grid_const
   using Sm = TcSmem<D>;
   uint64_t* bars = reinterpret_cast<uint64_t*>(sm + Sm::bar_off);
   uint64_t* bar_full = bars;                    // [STAGES]  TMA -> MMA
-  uint64_t* bar_empty = bars + TC_STAGES;       // [STAGES]  both warpgroups' MMAs done -> TMA
-  uint64_t* bar_users = bars + 2 * TC_STAGES;   // [1]
+  uint64_t* bar_empty = bars + Sh::STAGES;      // [STAGES]  both warpgroups' MMAs done -> TMA
+  uint64_t* bar_users = bars + 2 * Sh::STAGES;  // [1]
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
   const int q0 = blockIdx.x * a.ub;             // first query row of this CTA
   const int n_tiles = (a.n_items + TC_TN - 1) / TC_TN;
 
   if (threadIdx.x == 0) {
-    for (int s = 0; s < TC_STAGES; ++s) {
+    for (int s = 0; s < Sh::STAGES; ++s) {
       mbar_init(bar_full + s, 1);
       mbar_init(bar_empty + s, 2);  // one arrive per consumer warpgroup
     }
@@ -196,16 +222,20 @@ tc_score_kernel(const __grid_constant__ CUtensorMap tm_users, const __grid_const
     if (elect_one()) {
       tma_prefetch_desc(&tm_users);
       tma_prefetch_desc(&tm_items);
-      mbar_arrive_expect_tx(bar_users, Sh::USER_BYTES);
-      for (int c = 0; c < Sh::KC; ++c) tma_load_2d(sm + Sm::users_off + c * 16384, &tm_users, bar_users, c * 32, q0);
+      if constexpr (!Sh::US) {
+        mbar_arrive_expect_tx(bar_users, Sh::USER_BYTES);
+        for (int c = 0; c < Sh::KC; ++c) tma_load_2d(sm + Sm::users_off + c * 16384, &tm_users, bar_users, c * 32, q0);
+      }
       for (int n = 0; n < n_tiles * Sh::SPT; ++n) {  // ring stage n: tile n / SPT, k-chunks (n % SPT) * SC ...
-        const int s = n % TC_STAGES;
-        const uint32_t ph = (n / TC_STAGES) & 1;
+        const int s = n % Sh::STAGES;
+        const uint32_t ph = (n / Sh::STAGES) & 1;
         mbar_wait(bar_empty + s, ph ^ 1);  // first pass through the ring passes immediately
         mbar_arrive_expect_tx(bar_full + s, Sh::STAGE_BYTES);
         for (int c = 0; c < Sh::SC; ++c)
           tma_load_2d(sm + Sm::items_off + s * Sh::STAGE_BYTES + c * 16384, &tm_items, bar_full + s, ((n % Sh::SPT) * Sh::SC + c) * 32,
                       (n / Sh::SPT) * TC_TN);
+        if constexpr (Sh::US)  // the users' k-chunk n % SPT behind the item chunk
+          tma_load_2d(sm + Sm::items_off + s * Sh::STAGE_BYTES + 16384, &tm_users, bar_full + s, (n % Sh::SPT) * 32, q0);
       }
     }
     return;
@@ -356,21 +386,22 @@ tc_score_kernel(const __grid_constant__ CUtensorMap tm_users, const __grid_const
   };
   const uint32_t ua = smem_u32(sm + Sm::users_off + wg * 8192);
   const int w4 = warp & 3, g = lane >> 2, tq = lane & 3;
-  mbar_wait(bar_users, 0);
+  if constexpr (!Sh::US) mbar_wait(bar_users, 0);
   for (int t = 0; t < n_tiles; ++t) {
     float acc[64];
 #pragma unroll
     for (int p = 0; p < Sh::SPT; ++p) {
       const int n = t * Sh::SPT + p;
-      const int s = n % TC_STAGES;
-      mbar_wait(bar_full + s, (n / TC_STAGES) & 1);
+      const int s = n % Sh::STAGES;
+      mbar_wait(bar_full + s, (n / Sh::STAGES) & 1);
       const uint32_t ib = smem_u32(sm + Sm::items_off + s * Sh::STAGE_BYTES);
       wgmma_fence();
 #pragma unroll
       for (int c = 0; c < Sh::SC; ++c)
 #pragma unroll
-        for (int k = 0; k < 4; ++k)
-          wgmma_m64n128k8_tf32_ss(acc, make_smem_desc_k_sw128(ua + (p * Sh::SC + c) * 16384 + k * 32),
+        for (int k = 0; k < Sh::KS; ++k)
+          wgmma_m64n128k8_tf32_ss(acc,
+                                  make_smem_desc_k_sw128(Sh::US ? ib + 16384 + wg * 8192 + k * 32 : ua + (p * Sh::SC + c) * 16384 + k * 32),
                                   make_smem_desc_k_sw128(ib + c * 16384 + k * 32), (p | c | k) ? 1u : 0u);
       wgmma_commit();
       wgmma_wait<0>();
@@ -482,10 +513,18 @@ __global__ void __launch_bounds__(256) tc_rescore_kernel(const __grid_constant__
     if (mine[h]) {
       const float4* u = reinterpret_cast<const float4*>(w.ug + (size_t)q * D);
       const float4* it = reinterpret_cast<const float4*>(d.item_emb + (size_t)id[h] * D);
-      float4 iv[D / 4];  // the whole row in flight before the first fma: this kernel is bound by the latency of these gathers
+      // the whole row in flight before the first fma: this kernel is bound by the latency of these gathers.  D = 256
+      // takes the row in two pieces of 128 floats, so that its loads fit the registers without spilling
+      constexpr int P = D > 128 ? 128 : D;
+      float acc = 0.f;
 #pragma unroll
-      for (int c = 0; c < D / 4; ++c) iv[c] = __ldg(it + c);
-      s[h] = exact_score<D, D / 4>([&](int c) { return u[c]; }, [&](int c) { return iv[c]; });
+      for (int o = 0; o < D / 4; o += P / 4) {
+        float4 iv[P / 4];
+#pragma unroll
+        for (int c = 0; c < P / 4; ++c) iv[c] = __ldg(it + o + c);
+        acc = exact_score<P, P / 4>([&](int c) { return u[o + c]; }, [&](int c) { return iv[c]; }, acc);
+      }
+      s[h] = acc;
     }
   }
   // rank of my candidates by item id (ids are distinct; empty slots carry INT_MAX and never count)
@@ -764,7 +803,8 @@ static int launch_tc(const srb_topk_desc* d, const TcWorkspace& w, cudaStream_t 
 }
 
 int score_topk_tc(const srb_topk_desc* d, cudaStream_t st) {
-  SRB_REQUIRE(d->d == 64 || d->d == 128, "topk impl 2 (tensor cores) supports d=64 and d=128 only (got %d)", d->d);
+  SRB_REQUIRE(d->d == 16 || d->d == 32 || d->d == 64 || d->d == 128 || d->d == 256,
+              "topk impl 2 (tensor cores) supports d = 16, 32, 64, 128 and 256 only (got %d)", d->d);
   SRB_REQUIRE(d->k >= 1 && d->k <= TC_LONG_MAX, "topk impl 2: k=%d unsupported (1..%d)", d->k, TC_LONG_MAX);
   const int n_q = d->n_q;
   const TcWorkspace need = tc_carve(nullptr, n_q, d->n_items, d->d, d->k);
@@ -773,7 +813,13 @@ int score_topk_tc(const srb_topk_desc* d, cudaStream_t st) {
   SRB_REQUIRE(((uintptr_t)d->workspace & 255) == 0, "topk impl 2: workspace must be 256-byte aligned");
   SRB_REQUIRE(((uintptr_t)d->item_emb & 15) == 0, "topk impl 2: item_emb must be 16-byte aligned");
   const TcWorkspace w = tc_carve((char*)d->workspace, n_q, d->n_items, d->d, d->k);
-  return d->d == 64 ? launch_tc<64>(d, w, st) : launch_tc<128>(d, w, st);
+  switch (d->d) {
+    case 16: return launch_tc<16>(d, w, st);
+    case 32: return launch_tc<32>(d, w, st);
+    case 64: return launch_tc<64>(d, w, st);
+    case 128: return launch_tc<128>(d, w, st);
+    default: return launch_tc<256>(d, w, st);
+  }
 }
 
 }  // namespace srb
@@ -784,6 +830,17 @@ extern "C" int64_t srb_topk_fallback_count_offset(int32_t n_q, int32_t n_items) 
   if (n_q <= 0 || n_items <= 0) return -1;
   const srb::TcWorkspace w = srb::tc_carve((char*)256, n_q, n_items, 64, 1);
   return (int64_t)((char*)w.fb_count - (char*)256);
+}
+
+extern "C" float srb_topk_tc_error_bound(int32_t d) {
+  switch (d) {
+    case 16: return srb::TcShape<16>::E;
+    case 32: return srb::TcShape<32>::E;
+    case 64: return srb::TcShape<64>::E;
+    case 128: return srb::TcShape<128>::E;
+    case 256: return srb::TcShape<256>::E;
+    default: return -1.0f;
+  }
 }
 
 // O(n_q * cap(k) + n_items): the candidate buffers of long lists grow with k, never with the catalogue

@@ -547,7 +547,7 @@ def score_topk(user_emb, item_emb, users, rated_ptr, rated_idx, k, impl=0, stats
     if rated_ptr is not None:
         rated_ptr, rated_idx = _i32(rated_ptr, dev), _i32(rated_idx, dev)
         desc.rated_ptr, desc.rated_idx = _p(rated_ptr), _p(rated_idx)
-    if impl == 0:  # auto: tensor-core path for the embedding sizes it is written for, else the CUDA-core kernel
+    if impl == 0:  # auto: tensor-core path where it is measured faster, else the CUDA-core kernel
         impl = 2 if _tc_route(d, item_emb.shape[0], 0) else 1
     desc.k, desc.out_ids, desc.out_scores, desc.impl = k, _p(out_ids), _p(out_sc), impl
     ws = None
@@ -563,20 +563,24 @@ def score_topk(user_emb, item_emb, users, rated_ptr, rated_idx, k, impl=0, stats
 
 
 TOPK_KERNEL_MAX = 32  # list length of the selection kernels (one entry per lane)
-TOPK_TC_MAX = 256     # longest list of the tensor-core route (impl 2, d = 64 / 128)
+TOPK_TC_MAX = 256     # longest list of the tensor-core route (impl 2)
+TOPK_TC_WIDTHS = (16, 32, 64, 128, 256)       # embedding sizes impl 2 is built for
+TOPK_TC_AUTO_WIDTHS = (16, 32, 64, 128, 256)  # auto (impl 0) takes impl 2 for lists of up to 32 (DESIGN 9.4)
+TOPK_TC_LONG_AUTO_WIDTHS = (64, 128)          # ... and for lists of 33..256
 
 
 def long_list_route(d, n_items, k, impl=0):
     """True when score_topk ranks a list of k > 32 on the tensor cores (impl 2, candidate buffers behind a running
-    threshold) rather than from dense score rows (_score_topk_wide): d in {64, 128}, k <= 256, and from 1024 items on
-    unless impl 2 is asked for explicitly."""
-    return TOPK_KERNEL_MAX < int(k) <= TOPK_TC_MAX and _tc_route(d, n_items, impl)
+    threshold) rather than from dense score rows (_score_topk_wide): k <= 256, and either impl 2 asked for explicitly
+    (every width) or, under impl 0, d in {64, 128} from 1024 items on."""
+    return TOPK_KERNEL_MAX < int(k) <= TOPK_TC_MAX and _tc_route(d, n_items, impl, TOPK_TC_LONG_AUTO_WIDTHS)
 
 
-def _tc_route(d, n_items, impl):
-    """True when impl 2 (tensor cores) ranks at this width: d in {64, 128}, and either asked for explicitly or, under
-    impl 0 (auto), from 1024 items on."""
-    return int(d) in (64, 128) and (int(impl) == 2 or (int(impl) == 0 and int(n_items) >= 1024))
+def _tc_route(d, n_items, impl, auto_widths=TOPK_TC_AUTO_WIDTHS):
+    """True when impl 2 (tensor cores) ranks at this width: asked for explicitly, or under impl 0 (auto) at one of
+    auto_widths from 1024 items on."""
+    d, impl = int(d), int(impl)
+    return d in TOPK_TC_WIDTHS and (impl == 2 or (impl == 0 and d in auto_widths and int(n_items) >= 1024))
 
 
 def _score_topk_wide(user_emb, item_emb, users, rated_ptr, rated_idx, k):
