@@ -158,7 +158,9 @@ typedef struct srb_encoder_desc {
   uint64_t philox_offset;
   const int32_t* philox_step_dev;
   /* optional: the LAST layer is only evaluated for these rows (device list, duplicates allowed), e.g.
-   * the batch rows of a training step -- nothing else reads the final mean there */
+   * the batch rows of a training step -- nothing else reads the final mean there.  Refused with n_layers == 0
+   * and with cl_out set at layer_cl == n_layers: that last layer is needed in full, so leave last_rows unset and
+   * read the mean from final_out */
   const int32_t* last_rows;
   int32_t n_last_rows;
   const int32_t* last_rows_nv_dev; /* device-classified list: counts [5]; last_rows = 4 segments of n_last_rows (see srb_spmm_desc.n_vlong_dev) */
@@ -304,7 +306,8 @@ int srb_scatter_add_segments(float* dst, int32_t d, int32_t n_segs, const srb_sc
  * srb_adam_prepare: one tiny launch; increments the device step counter and writes
  *   scalars = {lr / (1 - beta1^t), sqrt(1 - beta2^t)} (double arithmetic, like torch's
  *   Python-float bias corrections).
- * srb_adam_step: p,m,v update from dense gradient g over n elements.
+ * srb_adam_step: p,m,v update from dense gradient g over n elements.  It and the SpMM's Adam epilogue round every
+ *   element as torch.optim.Adam's CUDA kernels do (bit for bit).
  * ------------------------------------------------------------------------------------- */
 int srb_adam_prepare(int32_t* step_dev, float* scalars_dev, double lr, double beta1,
                      double beta2, void* stream);

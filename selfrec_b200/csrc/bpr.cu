@@ -277,11 +277,7 @@ __global__ void __launch_bounds__(256) adam_step_kernel(float* __restrict__ p, f
   for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n4; i += stride) {
     float4 pp = reinterpret_cast<float4*>(p)[i], mm = reinterpret_cast<float4*>(m)[i], vv = reinterpret_cast<float4*>(v)[i];
     const float4 gg = reinterpret_cast<const float4*>(g)[i];
-#define SRB_ADAM1(F)                          \
-  mm.F = mm.F + w1 * (gg.F - mm.F);           \
-  vv.F = vv.F * b2;                           \
-  vv.F = vv.F + (w2 * gg.F) * gg.F;           \
-  pp.F = pp.F - step_size * (mm.F / (sqrtf(vv.F) / bc2_sqrt + eps));
+#define SRB_ADAM1(F) adam_elem(pp.F, mm.F, vv.F, gg.F, step_size, bc2_sqrt, w1, b2, w2, eps);
     SRB_ADAM1(x) SRB_ADAM1(y) SRB_ADAM1(z) SRB_ADAM1(w)
 #undef SRB_ADAM1
     reinterpret_cast<float4*>(p)[i] = pp;
@@ -290,12 +286,9 @@ __global__ void __launch_bounds__(256) adam_step_kernel(float* __restrict__ p, f
   }
   // scalar tail (n not a multiple of 4)
   for (long long i = n4 * 4 + (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += stride) {
-    float mm = m[i], vv = v[i];
-    const float gg = g[i];
-    mm = mm + w1 * (gg - mm);
-    vv = vv * b2;
-    vv = vv + (w2 * gg) * gg;
-    p[i] = p[i] - step_size * (mm / (sqrtf(vv) / bc2_sqrt + eps));
+    float pp = p[i], mm = m[i], vv = v[i];
+    adam_elem(pp, mm, vv, g[i], step_size, bc2_sqrt, w1, b2, w2, eps);
+    p[i] = pp;
     m[i] = mm;
     v[i] = vv;
   }

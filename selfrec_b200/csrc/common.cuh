@@ -152,6 +152,20 @@ __device__ __forceinline__ void adam_prepare(int32_t* step, float* scalars, doub
   scalars[1] = (float)sqrt(bc2);
 }
 
+// One Adam element, rounded as torch.optim.Adam's CUDA kernels round it (w1 = 1 - beta1, w2 = 1 - beta2):
+//   m.lerp_(g, w1)                      m = fma(w1, g - m, m)
+//   v.mul_(b2).addcmul_(g, g, w2)       v = fma(w2, g * g, v * b2), both products rounded first
+//   p.addcdiv_(m, denom, -step_size)    p = fma(-step_size, m / denom, p), denom = sqrt(v) / bc2_sqrt + eps
+// Round-to-nearest intrinsics pin every rounding: left to contraction, the compiler folded v * b2 into an fma (v off
+// torch's in a quarter of the elements) and fused the last multiply-subtract in some lanes of a kernel but not others.
+__device__ __forceinline__ void adam_elem(float& p, float& m, float& v, float g, float step_size, float bc2_sqrt, float w1,
+                                          float b2, float w2, float eps) {
+  m = __fmaf_rn(w1, __fsub_rn(g, m), m);
+  v = __fmaf_rn(w2, __fmul_rn(g, g), __fmul_rn(v, b2));
+  const float denom = __fadd_rn(__fdiv_rn(__fsqrt_rn(v), bc2_sqrt), eps);
+  p = __fmaf_rn(-step_size, __fdiv_rn(m, denom), p);
+}
+
 __device__ __forceinline__ float warp_sum(float v) {
 #pragma unroll
   for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(SRB_FULL_MASK, v, o);

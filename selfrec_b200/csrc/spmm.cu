@@ -142,11 +142,7 @@ __device__ __forceinline__ void spmm_epilogue(const SpmmArgs& a, int row, int gl
         float4 p4 = *reinterpret_cast<const float4*>(a.ap + o2);
         float4 m = *reinterpret_cast<const float4*>(a.am + o2);
         float4 v4 = *reinterpret_cast<const float4*>(a.av + o2);
-#define SRB_ADAM1(F)                                          \
-  m.F = m.F + a.w1 * (g.F - m.F);                             \
-  v4.F = v4.F * a.b2;                                         \
-  v4.F = v4.F + (a.w2 * g.F) * g.F;                           \
-  p4.F = p4.F - step_size * (m.F / (sqrtf(v4.F) / bc2_sqrt + a.aeps));
+#define SRB_ADAM1(F) adam_elem(p4.F, m.F, v4.F, g.F, step_size, bc2_sqrt, a.w1, a.b2, a.w2, a.aeps);
         SRB_ADAM1(x) SRB_ADAM1(y) SRB_ADAM1(z) SRB_ADAM1(w)
 #undef SRB_ADAM1
         st4(a.ap + o2, p4);
@@ -781,6 +777,10 @@ extern "C" int srb_encoder_forward(const srb_encoder_desc* e, void* stream) {
   SRB_REQUIRE(e->include_ego || e->n_layers > 0, "encoder: mean over zero layers");
   SRB_REQUIRE(!e->last_rows || (e->last_rows_out && e->last_rows_out != e->final_out && e->last_rows_out != e->E0),
               "encoder: last_rows needs a separate last_rows_out buffer");
+  // (with no layer, or with the last layer as the CL view, the last layer is the identity or runs in full, and the
+  // mean would land in final_out instead: refused rather than leave last_rows_out unwritten)
+  SRB_REQUIRE(!e->last_rows || (e->n_layers > 0 && !(e->cl_out && e->layer_cl == e->n_layers)),
+              "encoder: last_rows needs n_layers >= 1 and no CL view at the last layer");
   const size_t nd = (size_t)e->n * e->d;
   cudaStream_t st = (cudaStream_t)stream;
   const int L = e->n_layers;
