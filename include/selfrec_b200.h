@@ -208,11 +208,13 @@ typedef struct srb_bpr_desc {
   const int32_t* j_idx;
   const int32_t* b_dev; /* optional device batch size (<= b); NULL => b */
   int32_t b;
-  float emb_scale; /* gathered rows are emb_scale * emb[row] (lazy layer mean) */
+  float emb_scale; /* gathered rows are emb_scale * emb[row] (lazy layer mean); g_emb is the gradient w.r.t. these
+                    * scaled rows.  With l2_emb == emb the L2 term regularises the scaled rows; a separate l2_emb is
+                    * read unscaled */
   float reg;
   int32_t l2_terms;
   float l2_div;
-  float grad_scale; /* upstream dLoss (1.0) */
+  float grad_scale; /* upstream dLoss (1.0): scales g_emb and g_l2, not losses */
   float* losses;    /* [2] device */
   float* g_emb;
   float* g_l2;

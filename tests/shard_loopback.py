@@ -293,9 +293,9 @@ def _model_kw(edges, name, lcl, eps):
     return dict(eps=eps, tau=edges.TAU, cl_rate=edges.CL_RATE, layer_cl=lcl)
 
 
-def run_oracle_case(name, world, d, L, lcl=0, views=None):
+def run_oracle_case(name, world, d, L, lcl=0, views=None, reg=None):
     """Poison step, then test_gpu_step_edges' batch sequence against the float64 oracle (SimGCL / XSimGCL at eps = 0),
-    then the clean forward against the oracle's."""
+    then the clean forward against the oracle's.  reg: the L2 weight (test_gpu_step_edges.REG by default)."""
     import torch
     import oracle as orc
     import test_gpu_step_edges as edges
@@ -308,7 +308,8 @@ def run_oracle_case(name, world, d, L, lcl=0, views=None):
     rng = np.random.default_rng(d + L + world)
     E0 = (rng.standard_normal((U + I, d)) * 0.1).astype(np.float32)
     kw = _model_kw(edges, name, lcl, 0.0)
-    w = LoopbackWorld(world, lambda g: ShardedEngine(name, data, d, L, B, edges.LR, edges.REG, init_user=torch.from_numpy(E0[:U]),
+    reg = edges.REG if reg is None else float(reg)
+    w = LoopbackWorld(world, lambda g: ShardedEngine(name, data, d, L, B, edges.LR, reg, init_user=torch.from_numpy(E0[:U]),
                                                      init_item=torch.from_numpy(E0[U:]), group=g, device=dev, **kw), dev)
     w.assert_split_rows()
     view_csr = None
@@ -318,11 +319,12 @@ def run_oracle_case(name, world, d, L, lcl=0, views=None):
             e.set_view_graphs(*view_csr)
     es = w.engines
     state = [t for e in es for t in (e.user_emb, e.item_emb, e.mu, e.vu, e.mi, e.vi, e.step_dev, e.losses)]
-    tag = f"loopback W={world} {name}-d{d}-L{L}" + (f"-lcl{lcl}" if name == "XSimGCL" else "") + (f"-{views}" if views else "")
+    tag = f"loopback W={world} {name}-d{d}-L{L}" + (f"-lcl{lcl}" if name == "XSimGCL" else "") + (f"-{views}" if views else "") + \
+        (f" reg={reg:g}" if reg != edges.REG else "")
     t0 = time.time()
     edges._poison(torch, w, h["poison"], state, [t for e in es for t in (e.user_emb, e.item_emb)], workspaces=w.workspaces)
     print(f"{tag}: poison step done in {time.time() - t0:.1f} s", flush=True)
-    edges._run_sequence(torch, orc, h, name, d, L, lcl, view_csr, w.step, w.state, None, tag, eps=0.0, kappa=LB_KAPPA)
+    edges._run_sequence(torch, orc, h, name, d, L, lcl, view_csr, w.step, w.state, None, tag, eps=0.0, kappa=LB_KAPPA, reg=reg)
     print(f"{tag}: sequence done in {time.time() - t0:.1f} s", flush=True)
     # the clean forward against the oracle's, from the trained tables
     p = w.state()[0]

@@ -213,10 +213,10 @@ def _unambiguous_noise(orc, A, E0, noise):
     return noise
 
 
-def _run_sequence(torch, orc, hub, name, d, L, lcl, view_csr, run_step, read_state, noise_dev, tag, eps=EPS, kappa=KAPPA):
+def _run_sequence(torch, orc, hub, name, d, L, lcl, view_csr, run_step, read_state, noise_dev, tag, eps=EPS, kappa=KAPPA, reg=REG):
     """The batches after the poison step, each against the oracle, continuing from the device state every step.
     SimGCL / XSimGCL without noise_dev: the step's own noise at eps = 0, where the perturbation vanishes.  kappa: the
-    first-moment bar (KAPPA)."""
+    first-moment bar (KAPPA); reg: the L2 weight the engine was built with (REG)."""
     KAPPA = kappa
     rng = np.random.default_rng(d * 100 + L * 10 + lcl)
     A = hub["A"]
@@ -243,7 +243,7 @@ def _run_sequence(torch, orc, hub, name, d, L, lcl, view_csr, run_step, read_sta
         if b == 0:
             g = np.zeros((N, d))
         else:
-            ref = orc.train_step(name, A, p, U, u, i, j, n_layers=L, reg=REG, batch_size=B, eps=eps, tau=TAU, cl_rate=CL_RATE,
+            ref = orc.train_step(name, A, p, U, u, i, j, n_layers=L, reg=reg, batch_size=B, eps=eps, tau=TAU, cl_rate=CL_RATE,
                                  layer_cl=lcl, noise=noise, view_csr=view_csr)
             g = ref["grad"]
             for k, key in ((0, "rec"), (1, "l2")):
